@@ -1,6 +1,6 @@
 """Benchmark of the SONAR text-embedding hot path (BASELINE.json metric: sentences/sec -> 1024-d).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a engine
+    python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a engine
     python bench.py --impl reference --gpus N --steps K ...   # the CPU restatement of the reference path
 
 Workload (BASELINE.json configs[1]): text_sonar_basic_encoder architecture (24 layers, d=1024,
@@ -11,7 +11,7 @@ embed -> 24 encoder layers -> final LN -> mean-pool -> [4096,1024] fp32.
 * `value`  : whole-job sentences/s with the ids already resident in HBM (CUDA events, max over ranks)
 * `e2e`    : same metric through the reference-facing model call with HOST (pinned) ids in and
              HOST embeddings out, copies inside the timed region
-* `roofline`: the dominant kernel (tcgen05 GEMM, FFN inner-projection instantiation) timed alone
+* `roofline`: the dominant kernel (wgmma GEMM, FFN inner-projection instantiation) timed alone
              with CUDA events on its launch stream, against MEASURED_PEAKS.json
 * `cpu_baseline`: the fp32 PyTorch restatement of the fairseq2 op sequence (oracle/, "port") on the
              host cores, on a bounded sample of the same workload (rank 0, N=1 only)
@@ -22,6 +22,12 @@ embed -> 24 encoder layers -> final LN -> mean-pool -> [4096,1024] fp32.
 * `config5` : (N>1) BASELINE.json config 5 end to end: every rank encodes its shard of 1M/8 synthetic sentences,
              ONE NCCL all-gather assembles [N,1024], `xsim_distributed` mines it (ratio margin, k=4); predictions are
              checked against the fp64 oracle on rows of a 64K x 64K slice
+
+`--dump-outputs DIR` writes, after everything has been timed, what the timed paths returned as float32 `DIR/<name>.npy`:
+`sentence_embeddings` ([batch, 1024], the last timed step of the headline path) and, for the secondary blocks that ran,
+`speech_embeddings` [256, 1024], `decoder_tokens` / `decoder_scores` (best hypothesis per sentence, ids padded with -1) and
+`xsim_knn_indices` / `xsim_knn_values` [262144, 4] -- about 26 MB in all.  Weights and inputs are seeded, so two builds
+run with the same arguments can be compared output for output.
 """
 
 from __future__ import annotations
@@ -41,23 +47,22 @@ if ROOT not in sys.path:
 import torch  # noqa: E402
 
 BATCH, SEQ, D, FFN, LAYERS, HEADS, VOCAB = 4096, 128, 1024, 8192, 24, 16, 256206
-FALLBACK_PEAKS = {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0}
+# H100 SXM data-sheet figures (dense bf16, HBM3), used when no measured peaks file is present
+FALLBACK_PEAKS = {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0}
+
+
+# --dump-outputs: name -> float32 array of what a timed path returned; filled outside the timed regions, written at the end
+DUMP = None
+
+
+def keep_output(name: str, t) -> None:
+    if DUMP is not None:
+        DUMP[name] = t.detach().to(torch.float32).cpu().numpy()
 
 
 def flops_per_sentence(s: int) -> float:
     """SURVEY §8(d): F(S) = L*S*(2*(4d^2 + 2df) + 4*S*d)."""
     return LAYERS * s * (2.0 * (4 * D * D + 2 * D * FFN) + 4.0 * s * D)
-
-
-def kernel_source_digest() -> str:
-    """sha256 of the sources the dominant kernel is compiled from (ties an ncu capture to the code it measured)."""
-    import hashlib
-
-    h = hashlib.sha256()
-    for name in ("gemm_tcgen05.cu", "common.cuh", "sonar_b200_internal.h"):
-        with open(os.path.join(ROOT, "sonar_b200", "csrc", name), "rb") as f:
-            h.update(f.read())
-    return h.hexdigest()[:16]
 
 
 def load_peaks():
@@ -96,7 +101,7 @@ def synthetic_state_dict(device, layers=LAYERS, vocab=VOCAB, seed=1, std=0.02):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -317,7 +322,7 @@ def bench_speech(dev, peaks):
         return model(SequenceBatch(fb, PaddingMask(torch.tensor(fr), fb.shape[1], fr))).sentence_embeddings
 
     ms = _timed_ms(run, iters=3, warm=2)
-    # same-run A/B of the other relative-position attention kernel (tcgen05: attention_relpos_tc.cu)
+    # same-run A/B of the other relative-position attention kernel (wgmma: attention_relpos_tc.cu)
     other = "tcgen05" if model.attn_impl == "mma_sync" else "mma_sync"
     model_b = B200SpeechEncoderModel(sonar_speech_encoder_config("english"), sd, dev, attn_impl=other)
 
@@ -340,6 +345,7 @@ def bench_speech(dev, peaks):
                        non_blocking=True)
 
     ms_e2e = _timed_ms(run_e2e, iters=2, warm=1)
+    keep_output("speech_embeddings", run())
     flop_per_utt = 499 * 24 * 52.38e6 + 7e9  # SURVEY §8(d)
     peak = float(peaks["bf16_tflops_sustained"])
     val = n / ms * 1e3
@@ -415,6 +421,15 @@ def bench_decoder(dev, peaks):
         runs[label] = walls
     dt = min(runs["eager"][1:] + runs["cuda_graphs"][1:])
     steps = max(len(h[0].seq) for h in out.hypotheses if h)
+    if DUMP is not None:  # best hypothesis of every sentence from the last timed call
+        toks_out = torch.full((n, steps), -1.0)
+        scores_out = torch.full((n,), float("nan"))
+        for i, hyps in enumerate(out.hypotheses):
+            if hyps:
+                toks_out[i, : len(hyps[0].seq)] = torch.as_tensor(hyps[0].seq).float().cpu()
+                scores_out[i] = float(hyps[0].score)
+        keep_output("decoder_tokens", toks_out)
+        keep_output("decoder_scores", scores_out)
     # e2e: host embeddings in, host token sequences out (the generator's own D2H of hypotheses is inside every call)
     emb_host = emb.cpu().pin_memory()
     torch.cuda.synchronize()
@@ -455,7 +470,7 @@ def bench_decoder(dev, peaks):
     peak = float(peaks["bf16_tflops_sustained"])
     # the step is a SERIES of kernels with different bounds: the GEMMs against the tensor peak, the KV-cache attention against
     # HBM (every hypothesis row reads K and V of all earlier positions in all 24 layers: 2 * 2 B * D per position and layer)
-    hbm = float(peaks.get("hbm_gbs", FALLBACK_PEAKS.get("hbm_gbs", 6572.2)))
+    hbm = float(peaks.get("hbm_gbs", FALLBACK_PEAKS.get("hbm_gbs", 3350.0)))
     kv_bytes = n * beam * D * 4.0 * 24 * steps * (steps + 1) / 2.0
     floor_s = hyp_tokens * 1.63e9 / (peak * 1e12) + kv_bytes / (hbm * 1e9)
     del model, oracle, sd_cpu
@@ -508,6 +523,10 @@ def bench_xsim(dev, peaks):
     y = torch.randn((m, D), generator=g, device=dev)
     x = y + 0.1 * torch.randn((n, D), generator=g, device=dev) * y.norm(dim=1, keepdim=True) / 32.0  # §8(d) config 5
     ms = _timed_ms(lambda: xsim.knn(x, y, 4), iters=2, warm=1)
+    if DUMP is not None:
+        kv, ki = xsim.knn(x, y, 4)
+        keep_output("xsim_knn_values", kv)
+        keep_output("xsim_knn_indices", ki)  # < 2^24: exact in float32
     bidir_stats = {}
     ms_bidir = _timed_ms(lambda: xsim.knn_bidir(x, y, 4, bidir_stats), iters=2, warm=1)  # both directions from one pass
     err, _, pred = xsim.xsim(x[:65536], y[:65536], margin="ratio", k=4)
@@ -639,7 +658,6 @@ def main():
     ap.add_argument("--ln-fold", type=int, default=0, choices=[0, 1, 2],
                     help="0 = separate LayerNorm kernels (default schedule), 1 = LayerNorms folded into the GEMMs, "
                          "2 = only the attention-block LayerNorm folded")
-    ap.add_argument("--epi-groups", type=int, default=1, choices=[1, 2], help="epilogue warpgroups per GEMM CTA")
     ap.add_argument("--skip-cpu-baseline", action="store_true")
     ap.add_argument("--skip-secondary", action="store_true", help="N=1: skip the predict / speech / decoder / xsim blocks")
     ap.add_argument("--only", default="", help="N=1: comma list of secondary blocks to run (predict,speech,decoder,xsim)")
@@ -647,6 +665,8 @@ def main():
     ap.add_argument("--config5-per-gpu", type=int, default=125000, help="sentences every rank encodes for config 5")
     ap.add_argument("--layers", type=int, default=0, help="--impl reference only: reduced depth for the CPU test-suite")
     ap.add_argument("--vocab", type=int, default=0, help="--impl reference only: reduced vocabulary for the CPU test-suite")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the arrays the last timed step returned as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -654,7 +674,7 @@ def main():
 
     rank, world, local = dist_env()
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the sm_100a engine has no CPU path")
+        raise SystemExit("bench.py: no CUDA device; the sm_90a engine has no CPU path")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     dist = None
@@ -674,15 +694,15 @@ def main():
     B, S = args.batch, args.seq_len
     sd = synthetic_state_dict(dev)
     model = B200TextEncoderModel(sonar_text_encoder_config("basic"), sd, dev, cta_group=args.cta_group,
-                                 ln_fold=args.ln_fold, epi_groups=args.epi_groups)
-    # same-box A/B of the engine's schedule variants (clock and power state differ box to box by ~10 %, so variants are only
-    # comparable inside one run): (ln_fold, epi_groups)
+                                 ln_fold=args.ln_fold)
+    # same-run A/B of the engine's LayerNorm schedules (clock and power state differ from card to card, so variants are only
+    # comparable inside one run)
     variants = {}
     if rank == 0 and world == 1 and not args.skip_secondary:
-        for lf_, eg_ in ((0, 1), (0, 2), (2, 2), (1, 2)):
-            if (lf_, eg_) != (args.ln_fold, args.epi_groups):
-                variants[(lf_, eg_)] = B200TextEncoderModel(sonar_text_encoder_config("basic"), sd, dev,
-                                                            cta_group=args.cta_group, ln_fold=lf_, epi_groups=eg_)
+        for lf_ in (0, 2, 1):
+            if lf_ != args.ln_fold:
+                variants[lf_] = B200TextEncoderModel(sonar_text_encoder_config("basic"), sd, dev,
+                                                     cta_group=args.cta_group, ln_fold=lf_)
     sd_cpu = None
     if rank == 0 and world == 1 and not args.skip_cpu_baseline:
         sd_cpu = {k: v.cpu() for k, v in sd.items()}
@@ -722,8 +742,9 @@ def main():
             sampler.start()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
+        last = None
         for _ in range(steps):
-            fn()
+            last = fn()
         e1.record()
         torch.cuda.synchronize()
         if dist is not None:
@@ -733,27 +754,32 @@ def main():
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
         if dist is not None:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-        return float(ms.item()), clocks
+        return float(ms.item()), clocks, last
 
     # dominant kernel timed INSIDE the real steps: events recorded by the engine around the middle layer's FFN1 GEMM
     k_ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
     k_ev[0].record(); k_ev[1].record()  # materialise the handles
     model.profile_ffn1(*k_ev)
     # e2e is timed in two halves AROUND the resident loop so that the slow drift of the power-capped clock hits both
-    # measurements alike (round 1 timed them back to back and e2e came out faster than the copy-free value)
+    # measurements alike (timed back to back, e2e can come out faster than the copy-free value)
     k_a = args.steps // 2
     k_b = args.steps - k_a
     e2e_a = timed(step_e2e, k_a, args.warmup)[0] if k_a else 0.0
-    total_ms, clocks = timed(step_resident, args.steps, args.warmup, sample_clocks=True)
+    total_ms, clocks, last_out = timed(step_resident, args.steps, args.warmup, sample_clocks=True)
     in_step_kernel_ms = k_ev[0].elapsed_time(k_ev[1])  # the last timed step's launch
     model.profile_ffn1(None, None)
     e2e_b = timed(step_e2e, k_b, 1)[0]
     e2e_ms = e2e_a + e2e_b
+    global DUMP
+    if args.dump_outputs and rank == 0:
+        DUMP = {}
+        keep_output("sentence_embeddings", last_out)  # what the last timed step of the headline path returned
+    del last_out
     model.check_inputs()
     value = world * B * args.steps / (total_ms / 1e3)
     e2e_value = world * B * args.steps / (e2e_ms / 1e3)
 
-    # ---- dominant kernel alone: tcgen05 GEMM, FFN inner-projection instantiation (bias+ReLU, bf16 out) ----
+    # ---- dominant kernel alone: wgmma GEMM, FFN inner-projection instantiation (bias+ReLU, bf16 out) ----
     peaks, peak_kind = load_peaks()
     roofline = None
     if rank == 0:
@@ -778,22 +804,9 @@ def main():
         achieved = flops / (in_step_kernel_ms / 1e3) / 1e12  # the launch inside the last timed step
         peak = float(peaks.get("bf16_tflops_sustained", FALLBACK_PEAKS["bf16_tflops_sustained"]))
         burst = float(peaks.get("bf16_tflops", FALLBACK_PEAKS["bf16_tflops"]))
-        # DRAM bytes per launch of this kernel from an `ncu --set full` capture -- only quoted when the capture was taken
-        # on the kernel source being benched (the capture file records kernel_source_digest()), else null
-        traffic, traffic_note = None, None
-        tp = os.path.join(ROOT, "profiles", "ncu_gemm_ffn1.json")
-        if os.path.exists(tp) and (B, S) == (BATCH, SEQ):
-            with open(tp) as fh:
-                tj = json.load(fh)
-            if tj.get("kernel_source_digest") and tj.get("kernel_source_digest") == kernel_source_digest():
-                traffic = tj["dram_bytes_read"] + tj["dram_bytes_write"]
-                traffic_note = f"ncu capture {tj.get('capture')} of this kernel source (gemm_tcgen05.cu + common.cuh)"
-            else:
-                traffic_note = (f"null: the committed capture ({tj.get('capture')}) was taken on a different version of "
-                                "gemm_tcgen05.cu")
-        roofline = {"bound": "tensor", "kernel": "gemm_bf16_tcgen05_kernel<cta_group,EPI_BIAS_RELU,bf16> "
+        roofline = {"bound": "tensor", "kernel": "gemm_bf16_wgmma_kernel<cta_group,EPI_BIAS_RELU,bf16> "
                     f"M={T} N={FFN} K={D}", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                    "frac": achieved / peak, "traffic": traffic, "traffic_note": traffic_note,
+                    "frac": achieved / peak,
                     "ms_per_launch_in_step": in_step_kernel_ms,
                     "timed_alone": {"achieved": alone_tflops, "peak": burst, "frac": alone_tflops / burst,
                                     "peak_source": f"{peak_kind} bf16_tflops (burst)", "ms_per_launch": kms},
@@ -814,10 +827,10 @@ def main():
             torch.cuda.synchronize()
             return e0.elapsed_time(e1) / k
 
-        def vname(lf_, eg_):
-            return {0: "ln_separate", 1: "ln_folded", 2: "ln1_folded"}[lf_] + f"/epi_groups{eg_}"
+        def vname(lf_):
+            return {0: "ln_separate", 1: "ln_folded", 2: "ln1_folded"}[lf_]
 
-        allv = {(args.ln_fold, args.epi_groups): model, **variants}
+        allv = {args.ln_fold: model, **variants}
         for m in variants.values():
             run_n(m, 1)
         times = {k: [] for k in allv}
@@ -825,12 +838,12 @@ def main():
             for k, m in allv.items():
                 times[k].append(run_n(m, 3))
         ref_out = model(batch_dev).sentence_embeddings[:256].double()
-        ab = {"ms_per_step": {vname(*k): v for k, v in times.items()},
-              "sentences_per_s": {vname(*k): B / (sum(v) / len(v)) * 1e3 for k, v in times.items()},
-              "default": vname(args.ln_fold, args.epi_groups), "rel_l2_vs_default_max": {}}
+        ab = {"ms_per_step": {vname(k): v for k, v in times.items()},
+              "sentences_per_s": {vname(k): B / (sum(v) / len(v)) * 1e3 for k, v in times.items()},
+              "default": vname(args.ln_fold), "rel_l2_vs_default_max": {}}
         for k, m in variants.items():
             got = m(batch_dev).sentence_embeddings[:256].double()
-            ab["rel_l2_vs_default_max"][vname(*k)] = float(((got - ref_out).norm(dim=1) / ref_out.norm(dim=1)).max())
+            ab["rel_l2_vs_default_max"][vname(k)] = float(((got - ref_out).norm(dim=1) / ref_out.norm(dim=1)).max())
         variants.clear()
         allv.clear()
         torch.cuda.empty_cache()
@@ -913,13 +926,12 @@ def main():
             "data": "synthetic",
             "config": {"workload": f"text_sonar_basic_encoder arch (24L, d=1024, 16 heads, FFN 8192, vocab {VOCAB}), "
                                    f"batch {B} x seq_len {S} per GPU, random-init weights, synthetic ids",
-                       "l2": "inputs larger than L2 (per-step activations ~15 GB vs 126 MB L2)",
+                       "l2": "inputs larger than L2 (per-step activations ~15 GB vs 50 MB L2)",
                        "parallelism": f"dp{world}" + (" + all_gather of embeddings" if world > 1 else ""),
                        "cta_group": args.cta_group,
                        "layernorm": {0: "separate kernels", 1: "folded into the QKV / FFN1 GEMMs (statistics from the residual "
                                      "GEMMs' epilogues)", 2: "attention-block LayerNorm folded (FFN2 -> QKV), FFN-block LayerNorm "
-                                     "a kernel"}[args.ln_fold],
-                       "epi_groups": args.epi_groups},
+                                     "a kernel"}[args.ln_fold]},
             "clocks": clocks,
             "e2e": {"value": e2e_value, "unit": "sentences/s", "h2d_bytes_per_step": B * S * 8,
                     "d2h_bytes_per_step": B * D * 4, "ms_per_step": e2e_ms / args.steps},
@@ -932,6 +944,13 @@ def main():
         }
         if config5 is not None:
             line["config5"] = config5
+        if DUMP is not None:
+            import numpy as np
+
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for nme, arr in DUMP.items():
+                np.save(os.path.join(args.dump_outputs, nme + ".npy"), arr)
+            line["dumped_outputs"] = {nme: list(arr.shape) for nme, arr in DUMP.items()}
         print(json.dumps(line), flush=True)
     if dist is not None:
         dist.destroy_process_group()

@@ -1,4 +1,4 @@
-/* sonar_b200 -- C ABI of the B200-native SONAR text-embedding hot path.
+/* sonar_b200 -- C ABI of the Hopper-native SONAR text-embedding hot path.
  *
  * Plain C, no torch / CUDA types in the signatures: device buffers are `void*` /
  * typed raw pointers, the stream is an opaque `void*` (a `cudaStream_t`).
@@ -67,7 +67,7 @@ typedef struct SbEncoderConfig {
   int32_t pooling;       /* SB_POOL_* ; `basic` = SB_POOL_MEAN */
   float ln_eps;          /* 1e-5 */
   float embed_scale;     /* sqrt(model_dim) unless no_scale_embedding */
-  int32_t cta_group;     /* 0/2 = paired-CTA tcgen05 tiles (default), 1 = single-CTA */
+  int32_t cta_group;     /* 0/2 = CTA pairs (2-CTA clusters, W tile multicast; default), 1 = single CTAs */
   int32_t num_sms;       /* 0 = query the device */
   int32_t ln_fold;       /* 1 = fold every encoder-layer LayerNorm into the GEMMs around it (no LayerNorm kernel runs:
                           *     the residual GEMMs emit per-row statistics + a bf16 copy of the stream, the QKV / FFN1 GEMMs
@@ -75,9 +75,9 @@ typedef struct SbEncoderConfig {
                           *     prepares those weights in device memory it owns -- the caller's weights are not modified);
                           * 2 = fold only the attention-block LayerNorm (FFN2 emits, QKV applies); the FFN-block LayerNorm
                           *     stays a kernel (the out-projection is HBM-bound, its epilogue has no slack for the extra work);
-                          * 0 = separate LayerNorm kernels (the round-1 schedule) */
-  int32_t epi_groups;    /* 0/2 = two epilogue warpgroups per GEMM CTA (default); 1 = one (round-1 kernel, kept for A/B runs;
-                          *     needs ln_fold = 0) */
+                          * 0 = separate LayerNorm kernels */
+  int32_t epi_groups;    /* 0, 1 or 2; accepted for compatibility (1 needs ln_fold = 0 and CTA pairs): the Hopper GEMM
+                          *     has one epilogue schedule */
 } SbEncoderConfig;
 
 /* All pointers are DEVICE pointers and stay owned by the caller (must outlive the handle).
@@ -173,7 +173,7 @@ int sb_gemm_residual_splitk(const void* A, int64_t lda, const void* W, int64_t l
 
 /* C[M,N] = epi(A[M,K] * W[N,K]^T + bias[N]) ; A, W bf16 row-major; C bf16 (out_fp32=0) or fp32;
  * residual (SB_EPI_BIAS_RESIDUAL) has C's dtype and may alias C.  N % 256 == 0, K % 64 == 0.
- * cta_group: 2 = paired-CTA tcgen05 tiles, 1 = single-CTA tiles, 0 = automatic (paired tiles, except that M <= 64 with
+ * cta_group: 2 = CTA-pair tiles (2-CTA clusters), 1 = single-CTA tiles, 0 = automatic (paired tiles, except that M <= 64 with
  * K % 256 == 0 takes the weight-streaming mma.sync path the decoder step uses; then only N % 8 == 0 is required). */
 int sb_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc, int32_t out_fp32,
                  const float* bias, const void* residual, int64_t ldr, int32_t M, int32_t N, int32_t K, int32_t epi,
@@ -184,7 +184,7 @@ int sb_layernorm(const float* x, const float* gamma, const float* beta, float ep
                  void* stream);
 
 /* packed self-attention: qkv bf16 [total_tokens, 3*64*H], cu_seqlens DEVICE int32 [B+1], out bf16 [total_tokens, 64*H].
- * impl 0 = auto (= 2), 1 = mma.sync flash kernel (kept for tests / A-B timing), 2 = tcgen05 (any length; 128-key
+ * impl 0 = auto (= 2), 1 = mma.sync flash kernel (kept for tests / A-B timing), 2 = wgmma (any length; 128-key
  * tiles with online softmax beyond 128 tokens). */
 int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t max_len, int32_t H,
                  int64_t total_tokens, int32_t impl, void* out, void* stream);
@@ -296,8 +296,8 @@ typedef struct SbSpeechConfig {
   int32_t pooler_layers;        /* 3 (english) / 6 (non_english) */
   int32_t pooler_ffn_inner_dim; /* 4096 */
   float ln_eps;                 /* 1e-5 */
-  int32_t attn_impl;            /* relative-position attention: 0 = tcgen05 kernel, 1 = mma.sync kernel (the Python wrapper's
-                                 * default: measured faster end to end, see DESIGN.md §7) */
+  int32_t attn_impl;            /* relative-position attention: 0 = wgmma kernel, 1 = mma.sync kernel (the Python wrapper's
+                                 * default) */
 } SbSpeechConfig;
 
 /* every field is a DEVICE pointer (matrices bf16 [out,in]; vectors fp32) */
@@ -365,7 +365,7 @@ int sb_xsim_workspace_bytes(int32_t n, int32_t m, int32_t d, size_t* bytes);
 
 /* k nearest rows of y[m,d] (cosine) for every row of x[n,d]; x, y DEVICE fp32 row-major (raw, un-normalised).
  * out_val DEVICE fp64 [n,k] exact cosines, out_idx DEVICE int32 [n,k]; sorted by (cosine desc, index asc).
- * Candidates come from a bf16 tcgen05 GEMM with a fused running top-16, then are re-scored in fp64. */
+ * Candidates come from a bf16 wgmma GEMM with a fused running top-16, then are re-scored in fp64. */
 int sb_xsim_knn(const float* x, const float* y, int32_t n, int32_t m, int32_t d, int32_t k, double* out_val,
                 int32_t* out_idx, void* workspace, size_t workspace_bytes, void* stream);
 

@@ -1,4 +1,4 @@
-"""sonar_b200 -- B200-native (sm_100a) engine behind the SONAR ``inference_pipelines`` API.
+"""sonar_b200 -- Hopper (sm_90a) engine behind the SONAR ``inference_pipelines`` API.
 
 Only the text-embedding hot path lives here (SURVEY.md §8): host batcher + pipeline mirror
 in Python, all arithmetic in ``lib/libsonar_b200.so`` (``include/sonar_b200.h``).

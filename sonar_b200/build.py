@@ -1,8 +1,8 @@
-"""In-tree build of the sm_100a CUDA library (``sonar_b200/lib/libsonar_b200.so``).
+"""In-tree build of the sm_90a CUDA library (``sonar_b200/lib/libsonar_b200.so``).
 
-nvcc cross-compiles without a GPU.  The explicit ``-gencode arch=compute_100a,code=sm_100a``
-form is required: a bare ``-arch=sm_100a`` also emits a ``compute_100`` PTX pass in which
-``tcgen05.*`` does not assemble.
+nvcc cross-compiles without a GPU.  The explicit ``-gencode arch=compute_90a,code=sm_90a``
+form is required: a bare ``-arch=sm_90a`` also emits a ``compute_90`` PTX pass in which
+``wgmma.*`` does not assemble.
 """
 
 from __future__ import annotations
@@ -18,11 +18,11 @@ ROOT = Path(__file__).resolve().parent
 CSRC = ROOT / "csrc"
 LIB_DIR = ROOT / "lib"
 LIB_PATH = LIB_DIR / "libsonar_b200.so"
-SOURCES = ["encoder.cu", "gemm_tcgen05.cu", "gemm_skinny.cu", "attention.cu", "attention_tc.cu", "elementwise.cu", "xsim.cu", "decoder.cu", "beam.cu", "fbank.cu", "conformer.cu", "attention_relpos_tc.cu"]
+SOURCES = ["encoder.cu", "gemm_wgmma.cu", "gemm_skinny.cu", "attention.cu", "attention_tc.cu", "elementwise.cu", "xsim.cu", "decoder.cu", "beam.cu", "fbank.cu", "conformer.cu", "attention_relpos_tc.cu"]
 HEADERS = ["common.cuh", "sonar_b200_internal.h", "../../include/sonar_b200.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -49,7 +49,7 @@ def _digest() -> str:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every CUDA source for sm_100a into one shared library (incremental:
+    """Compile every CUDA source for sm_90a into one shared library (incremental:
     skipped when sources + flags hash matches the stamp next to the library)."""
     LIB_DIR.mkdir(exist_ok=True)
     stamp = LIB_DIR / "build.stamp"
@@ -73,7 +73,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError(f"nvcc failed on {name}")
         objs.append(str(obj))
-    cmd = [nvcc, "-shared", "-o", str(LIB_PATH), *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", str(LIB_PATH), *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     log_lines += ["$ " + " ".join(cmd), r.stdout, r.stderr]
     if r.returncode != 0:

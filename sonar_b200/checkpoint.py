@@ -1,4 +1,4 @@
-"""Checkpoint converters: legacy fairseq layouts -> the fairseq2 state-dict names the B200 models consume.
+"""Checkpoint converters: legacy fairseq layouts -> the fairseq2 state-dict names the CUDA models consume.
 
 Host-side mirrors of the reference's converters (pure key renaming + one row permutation, no arithmetic):
 

@@ -6,13 +6,13 @@
 // (sonar/models/sonar_text/factory.py:130-141) = F.scaled_dot_product_attention with
 // a key-padding mask, scale 1/sqrt(head_dim), no causal mask (SURVEY App. A.2, F4).
 //
-// NOT on the product path any more (attention_tc.cu handles every length on tcgen05); kept as `impl = 1` of
+// NOT on the product path any more (attention_tc.cu handles every length on wgmma); kept as `impl = 1` of
 // sb_attention: an independent second implementation for tests and A/B timing.
 // mma.sync.m16n8k16 bf16 (legacy tensor path), flash-style online softmax.
 // One CTA = one (sequence, head, 128-query block); 8 warps x 16 query rows; K/V are
 // streamed in 64-key blocks through swizzled shared memory with cp.async.
 // At S=128 this op is ~1.2% of the encoder FLOPs and HBM-bound (reads 6 B/token/dim,
-// writes 2); the tcgen05 version is tracked in DESIGN.md.
+// writes 2); the wgmma kernel is described in DESIGN.md.
 
 #include "common.cuh"
 #include "sonar_b200_internal.h"
@@ -232,7 +232,7 @@ int attention_packed(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B,
     set_last_error("attention_packed: unsupported B=%d H=%d", B, H);
     return -1;
   }
-  // impl 0 (auto) and 2: the tcgen05 kernel, any sequence length (128-key tiles with online softmax beyond 128 tokens);
+  // impl 0 (auto) and 2: the wgmma kernel, any sequence length (128-key tiles with online softmax beyond 128 tokens);
   // impl 1 keeps the mma.sync flash kernel below reachable for A/B measurements and as a second implementation in tests
   if (impl != 1) return attention_packed_tc(qkv, cu_seqlens, B, H, total_tokens, out, num_sms, stream);
   dim3 grid((unsigned)((max_len + kQBlock - 1) / kQBlock), (unsigned)H, (unsigned)B);

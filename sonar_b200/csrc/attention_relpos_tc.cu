@@ -1,4 +1,4 @@
-// Transformer-XL relative-position self-attention of the w2v-BERT Conformer blocks on tcgen05 (BASELINE.json config 3,
+// Transformer-XL relative-position self-attention of the w2v-BERT Conformer blocks on wgmma (BASELINE.json config 3,
 // SURVEY §8 row a11 / App. B.2; reference wiring sonar/models/sonar_speech/factory.py:64-71, parameter names
 // sdpa.u_bias / sdpa.v_bias / sdpa.r_proj in sonar_speech/handler.py:81-83):
 //
@@ -6,26 +6,21 @@
 //
 // over PACKED utterances (row = cu[b] + t), keys >= len get probability exactly 0.
 //
-// Work decomposition.  An ITEM is (utterance b, 128-query tile, head h); a UNIT is one 128-key tile of it:
-//     S1[128 x 128] = Qu . K^T                      Qu = bf16(q + u), Qv = bf16(q + v): prepared once per layer by
-//     B [128 x 256] = Qv . Pw^T                     relpos_qprep_kernel, so no bias vector is added inside this kernel
+// Work decomposition.  An ITEM is (utterance b, 128-query tile, head h); a UNIT is one 128-key tile of it; each of the two
+// consumer warpgroups owns 64 query rows (w = 0, 1) of the unit:
+//     S1[64 x 128] = Qu . K^T                       Qu = bf16(q + u), Qv = bf16(q + v): prepared once per layer by
+//     Bw[64 x 192] = Qv . Pw^T                      relpos_qprep_kernel, so no bias vector is added inside this kernel
 //       Pw = the 256 rows of p the tile can reach: row n0 + cB, n0 = c - 1 - (q0 + 127) + j0, and the score of (query il,
 //       key jl) of the tile uses column cB = 127 - il + jl -- the Transformer-XL "shift": every query row reads B at its
-//       own offset.  TMEM loads are warp-uniform in the column address, so the 32-column window a warp fetches covers its
-//       32 rows' needs (63 columns) and each thread then shifts its row by s = 31 - lane with a 5-stage barrel shifter of
-//       register selects (16, 8, 4, 2, 1) -- no shared-memory round trip, no bank conflicts.
-//     P = exp2((S1 + shift(B) - m_ref) / 8 * log2 e) one thread per query row; m_ref is a lazily raised reference (see the
-//                                                   softmax section), so the scores are read once and exponentiated at once
-//     O[128 x 64]  = P . V                          P stays in tensor memory (tcgen05.st + A-from-TMEM MMA)
-// Tensor memory holds 256 columns per softmax group: S1 (128) | B half (128).  B is produced in two halves (columns
-// 0-127, then 128-255 into the same TMEM columns): a chunk of 32 keys takes its position term from the low half when
-// jl <= il and from the high half otherwise, so pass A completes the score chunks c < warp, pass B the chunks c >= warp (the
-// diagonal chunk keeps its 32 low-half columns in registers in between); the probabilities overwrite the chunk's own score
-// columns and O later reuses the B columns.  Two softmax warpgroups per CTA (one persistent CTA per SM) work on different items, so one group's
-// exponentials overlap the other's MMAs; each group has its own operand slots and its own TMA producer thread.
-//
-// Warps: 0 = producer of group 0, 3 = producer of group 1, 1 = MMA issuer (event driven over both groups), 2 = TMEM allocator,
-// 4-7 / 8-11 = softmax groups 0 / 1 (TMEM lane quarter = warp % 4).
+//       own offset.  Warpgroup w needs cB in [64 - 64 w, 254 - 64 w], i.e. 192 rows of Pw from row 64 - 64 w, and its
+//       query row rl then reads column 63 - rl + jl of Bw.  The accumulator layout of wgmma fixes which thread holds which
+//       column, so Bw goes through a shared-memory buffer (fp32, row stride 197 floats: the skewed reads and the fragment
+//       writes are at most 2-way bank conflicted) in two 96-column halves and every thread gathers the position terms of
+//       its S1 fragment from there.
+//     P = exp2((S1 + shift(B) - m) / 8 * log2 e)    online softmax on the accumulator fragments (a row = 4 lanes)
+//     O[64 x 64] += P . V                           A = P from registers, V the MN-major B operand
+// Warpgroup 0 = TMA producer (one thread); Qu | Qv stay for the item, K | Pw and V are single slots that are released as
+// soon as the products reading them have retired, so the next unit's loads run under this unit's softmax.
 
 #include "common.cuh"
 #include "sonar_b200_internal.h"
@@ -36,22 +31,17 @@ namespace sb {
 namespace {
 
 constexpr int kTile = 128 * 64 * 2;              // one [128 x 64] bf16 operand tile = 16 KB
-constexpr int kGroupBytes = 6 * kTile;            // per softmax group: Qu | Qv | K | P_lo | P_hi | V  (96 KB)
-constexpr int kOffQu = 0, kOffQv = kTile, kOffK = 2 * kTile, kOffPlo = 3 * kTile, kOffPhi = 4 * kTile, kOffV = 5 * kTile;
+constexpr int kOperandBytes = 6 * kTile;          // Qu | Qv | K | P_lo | P_hi | V  (96 KB)
+constexpr int kOffQu = 0, kOffQv = kTile, kOffK = 2 * kTile, kOffPlo = 3 * kTile, kOffV = 5 * kTile;
+constexpr int kBLd = 197;                         // floats per row of a warpgroup's Bw buffer (192 + skew padding)
+constexpr int kBBytes = 64 * kBLd * 4;            // per consumer warpgroup
 constexpr int kBarBytes = 512;
 constexpr int kMaxBatch = 2047;                   // cu_seqlens and the query-tile prefix are staged in shared memory
-constexpr int kSmemBytes = 2 * kGroupBytes + kBarBytes + 2 * (kMaxBatch + 1) * 4 + 1024;
+constexpr int kSmemBytes = kOperandBytes + 2 * kBBytes + kBarBytes + 2 * (kMaxBatch + 1) * 4 + 1024;
 constexpr int kThreads = 384;
-static_assert(kSmemBytes <= 232448, "shared memory budget");
+static_assert(kSmemBytes <= 232448, "shared memory budget of one sm_90 block");
 
-// barriers of one softmax group
-enum { Q_FULL = 0, Q_EMPTY, KP_FULL, KP_EMPTY, V_FULL, V_EMPTY, AB_FULL, A_DONE, BHI_FULL, P_READY, O_FULL, O_FREE, kNumBars };
-
-__device__ __forceinline__ uint64_t desc_mnmajor_sw128(uint32_t smem_addr) {  // V as the MN-major B operand (see attention_tc.cu)
-  uint64_t lo = ((smem_addr >> 4) & 0x3FFFu) | (uint64_t((128u * 128u) >> 4) << 16);
-  uint64_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-  return lo | (hi << 32);
-}
+enum { Q_FULL = 0, Q_EMPTY, KP_FULL, KP_EMPTY, V_FULL, V_EMPTY, kNumBars };
 
 __device__ __forceinline__ float ex2f(float x) {
   float y;
@@ -59,19 +49,7 @@ __device__ __forceinline__ float ex2f(float x) {
   return y;
 }
 
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-
-// The unit sequence of one softmax group: items first + i * stride; an item = (query tile, head) of one utterance, expanded
+// The unit sequence of this CTA: items first + i * stride; an item = (query tile, head) of one utterance, expanded
 // into its key tiles.  tile_cu[b] = number of query tiles before utterance b.
 struct RelStream {
   const int32_t* cu;
@@ -107,64 +85,34 @@ struct RelStream {
   }
 };
 
-// lo[k] = in[k + s], k = 0..31, s in [0, 31], where in = lo | hi (64 values): five select stages (16, 8, 4, 2, 1), in place.
-// (Two separate 32-register arrays with compile-time indices only: nothing here may end up in local memory.)
-template <int SH>
-__device__ __forceinline__ void barrel_stage(uint32_t (&lo)[32], uint32_t (&hi)[32], bool on) {
-  // after this stage positions [0, 64 - sum of shifts so far) are meaningful; ascending k reads only not-yet-written slots
-#pragma unroll
-  for (int k = 0; k < 32; ++k) {
-    const uint32_t src = (k + SH < 32) ? lo[(k + SH) & 31] : hi[(k + SH - 32) & 31];
-    lo[k] = on ? src : lo[k];
-  }
-#pragma unroll
-  for (int k = 0; k + SH < 32; ++k) hi[k] = on ? hi[k + SH] : hi[k];
-}
-__device__ __forceinline__ void barrel_shift(uint32_t (&lo)[32], uint32_t (&hi)[32], int s) {
-  barrel_stage<16>(lo, hi, s & 16);
-  barrel_stage<8>(lo, hi, s & 8);
-  barrel_stage<4>(lo, hi, s & 4);
-  barrel_stage<2>(lo, hi, s & 2);
-  barrel_stage<1>(lo, hi, s & 1);
-}
-
 __global__ void __launch_bounds__(kThreads, 1)
 attention_relpos_tc_kernel(const __grid_constant__ CUtensorMap tm_qu, const __grid_constant__ CUtensorMap tm_qv,
                            const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_p,
                            const int32_t* cu_g, int B, int H, int S_center, __nv_bfloat16* __restrict__ out) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * kGroupBytes);  // [2][kNumBars]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * kNumBars);
-  int32_t* cu = reinterpret_cast<int32_t*>(smem + 2 * kGroupBytes + kBarBytes);
+  float* smem_bw = reinterpret_cast<float*>(smem + kOperandBytes);  // [2][64][kBLd]
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kOperandBytes + 2 * kBBytes);  // [kNumBars]
+  int32_t* cu = reinterpret_cast<int32_t*>(smem + kOperandBytes + 2 * kBBytes + kBarBytes);
   int32_t* tile_cu = cu + (kMaxBatch + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg_idx = threadIdx.x >> 7;
   const int D = H * 64;
   for (int i = threadIdx.x; i <= B; i += kThreads) cu[i] = cu_g[i];
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_qu);
     tma_prefetch_desc(&tm_qv);
     tma_prefetch_desc(&tm_qkv);
     tma_prefetch_desc(&tm_p);
-    for (int g = 0; g < 2; ++g) {
-      uint64_t* b = bars + g * kNumBars;
-      mbar_init(&b[Q_FULL], 1);
-      mbar_init(&b[Q_EMPTY], 1);
-      mbar_init(&b[KP_FULL], 1);
-      mbar_init(&b[KP_EMPTY], 1);
-      mbar_init(&b[V_FULL], 1);
-      mbar_init(&b[V_EMPTY], 1);
-      mbar_init(&b[AB_FULL], 1);
-      mbar_init(&b[A_DONE], 4);
-      mbar_init(&b[BHI_FULL], 1);
-      mbar_init(&b[P_READY], 4);
-      mbar_init(&b[O_FULL], 1);
-      mbar_init(&b[O_FREE], 4);
-    }
+    mbar_init(&bar[Q_FULL], 1);
+    mbar_init(&bar[Q_EMPTY], 8);   // one arrive per consumer warp
+    mbar_init(&bar[KP_FULL], 1);
+    mbar_init(&bar[KP_EMPTY], 8);
+    mbar_init(&bar[V_FULL], 1);
+    mbar_init(&bar[V_EMPTY], 8);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<1>(tmem_ptr_smem, 512);
   __syncthreads();
   if (threadIdx.x == 0) {  // query-tile prefix over the utterances (B <= kMaxBatch)
     int acc = 0;
@@ -174,288 +122,203 @@ attention_relpos_tc_kernel(const __grid_constant__ CUtensorMap tm_qu, const __gr
     }
     tile_cu[B] = acc;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  if ((warp == 0 || warp == 3) && lane == 0) {
-    // ============================ TMA producer of group g ============================
-    const int g = (warp == 0) ? 0 : 1;
-    uint64_t* bar = bars + g * kNumBars;
-    uint8_t* base = smem + g * kGroupBytes;
-    RelStream s;
-    s.init(cu, tile_cu, B, H, blockIdx.x + g * gridDim.x, 2 * gridDim.x);
-    uint32_t n = 0, ni = 0;  // units / items loaded so far
-    while (s.valid) {
-      const int col = s.h * 64;
-      if (s.kt == 0) {  // the item's biased queries
-        mbar_wait(&bar[Q_EMPTY], (ni & 1) ^ 1);
-        mbar_arrive_expect_tx(&bar[Q_FULL], 2 * kTile);
-        tma_load_2d(base + kOffQu, &tm_qu, &bar[Q_FULL], col, s.tok0 + s.q0);
-        tma_load_2d(base + kOffQv, &tm_qv, &bar[Q_FULL], col, s.tok0 + s.q0);
-        ++ni;
-      }
-      const int j0 = s.kt * 128;
-      const int n0 = S_center - 1 - (s.q0 + 127) + j0;  // p row of window column 0 (may be negative: zero filled)
-      mbar_wait(&bar[KP_EMPTY], (n & 1) ^ 1);
-      mbar_arrive_expect_tx(&bar[KP_FULL], 3 * kTile);
-      tma_load_2d(base + kOffK, &tm_qkv, &bar[KP_FULL], D + col, s.tok0 + j0);
-      tma_load_2d(base + kOffPlo, &tm_p, &bar[KP_FULL], col, n0);
-      tma_load_2d(base + kOffPhi, &tm_p, &bar[KP_FULL], col, n0 + 128);
-      mbar_wait(&bar[V_EMPTY], (n & 1) ^ 1);
-      mbar_arrive_expect_tx(&bar[V_FULL], kTile);
-      tma_load_2d(base + kOffV, &tm_qkv, &bar[V_FULL], 2 * D + col, s.tok0 + j0);
-      ++n;
-      s.advance();
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ============================ MMA issuer: event driven over both groups ============================
-    constexpr uint32_t idesc_s = umma_idesc_bf16_f32(128, 128);
-    constexpr uint32_t idesc_o = umma_idesc_bf16_f32(128, 64) | (1u << 16);  // B operand MN-major
-    RelStream s0, s1;
-    s0.init(cu, tile_cu, B, H, blockIdx.x, 2 * gridDim.x);
-    s1.init(cu, tile_cu, B, H, blockIdx.x + gridDim.x, 2 * gridDim.x);
-    int ph0 = s0.valid ? 0 : 3, ph1 = s1.valid ? 0 : 3;  // next phase of each group (3 = stream exhausted)
-    uint32_t n0u = 0, n1u = 0, ni0 = 0, ni1 = 0;          // units / items issued per group
-    long long t_idle = clock64();
-    while (ph0 != 3 || ph1 != 3) {
-      bool progressed = false;
-#pragma unroll
-      for (int g = 0; g < 2; ++g) {
-        const int ph = g ? ph1 : ph0;
-        if (ph == 3) continue;
-        const uint32_t n = g ? n1u : n0u;
-        const uint32_t ni = g ? ni1 : ni0;
-        const int kt = g ? s1.kt : s0.kt;
-        const int nt = g ? s1.nt : s0.nt;
-        const int len = g ? s1.len : s0.len;
-        uint64_t* bar = bars + g * kNumBars;
-        const uint32_t sbase = smem_u32(smem + g * kGroupBytes);
-        const uint32_t tS = tmem_base + g * 256, tB = tS + 128;
-        if (ph == 0) {  // S1 = Qu K^T, B_lo = Qv P_lo^T
-          if (kt == 0 && !mbar_test_wait(&bar[Q_FULL], ni & 1)) continue;
-          if (!mbar_test_wait(&bar[KP_FULL], n & 1)) continue;
-          if (n > 0 && !mbar_test_wait(&bar[O_FREE], (n - 1) & 1)) continue;
-          tc_fence_after();
-          const uint64_t qu = umma_desc_kmajor_sw128(sbase + kOffQu), qv = umma_desc_kmajor_sw128(sbase + kOffQv);
-          const uint64_t kd = umma_desc_kmajor_sw128(sbase + kOffK), pl = umma_desc_kmajor_sw128(sbase + kOffPlo);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16<1>(tS, qu + uint64_t(2 * k), kd + uint64_t(2 * k), idesc_s, k != 0);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16<1>(tB, qv + uint64_t(2 * k), pl + uint64_t(2 * k), idesc_s, k != 0);
-          umma_commit<1>(&bar[AB_FULL]);
-          if (g) ph1 = 1; else ph0 = 1;
-          progressed = true;
-        } else if (ph == 1) {  // B_hi = Qv P_hi^T over the same TMEM columns, once pass A has consumed B_lo
-          if (!mbar_test_wait(&bar[A_DONE], n & 1)) continue;
-          tc_fence_after();
-          const uint64_t qv = umma_desc_kmajor_sw128(sbase + kOffQv), phd = umma_desc_kmajor_sw128(sbase + kOffPhi);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16<1>(tB, qv + uint64_t(2 * k), phd + uint64_t(2 * k), idesc_s, k != 0);
-          umma_commit<1>(&bar[BHI_FULL]);
-          umma_commit<1>(&bar[KP_EMPTY]);                    // K, P_lo, P_hi are dead
-          if (kt == nt - 1) umma_commit<1>(&bar[Q_EMPTY]);   // last key tile of the item: Qu, Qv are dead too
-          if (g) ph1 = 2; else ph0 = 2;
-          progressed = true;
-        } else {  // O = P V  (P over the score columns, O into B+0..63)
-          if (!mbar_test_wait(&bar[P_READY], n & 1)) continue;
-          if (!mbar_test_wait(&bar[V_FULL], n & 1)) continue;
-          tc_fence_after();
-          const int kv_valid = min(128, len - kt * 128);
-          const int ksteps = (kv_valid + 15) >> 4;
-          for (int k = 0; k < ksteps; ++k)  // 16 keys per k-step: P of key chunk c lives at S columns 32c .. 32c+15
-            umma_bf16_ts(tB, tS + 32 * (k >> 1) + 8 * (k & 1), desc_mnmajor_sw128(sbase + kOffV + k * 2048), idesc_o, k != 0);
-          umma_commit<1>(&bar[O_FULL]);
-          umma_commit<1>(&bar[V_EMPTY]);
-          if (g) {
-            ++n1u;
-            if (kt == nt - 1) ++ni1;
-            s1.advance();
-            ph1 = s1.valid ? 0 : 3;
-          } else {
-            ++n0u;
-            if (kt == nt - 1) ++ni0;
-            s0.advance();
-            ph0 = s0.valid ? 0 : 3;
-          }
-          progressed = true;
+
+  RelStream u;
+  u.init(cu, tile_cu, B, H, blockIdx.x, gridDim.x);
+  uint32_t n = 0, ni = 0;  // units / items so far
+
+  if (wg_idx == 0) {
+    // ============================ TMA producer ============================
+    if (warp == 0 && lane == 0) {
+      while (u.valid) {
+        const int col = u.h * 64;
+        if (u.kt == 0) {  // the item's biased queries
+          mbar_wait(&bar[Q_EMPTY], (ni & 1) ^ 1);
+          mbar_arrive_expect_tx(&bar[Q_FULL], 2 * kTile);
+          tma_load_2d(smem + kOffQu, &tm_qu, &bar[Q_FULL], col, u.tok0 + u.q0);
+          tma_load_2d(smem + kOffQv, &tm_qv, &bar[Q_FULL], col, u.tok0 + u.q0);
+          ++ni;
         }
-      }
-      if (progressed) {
-        t_idle = clock64();
-      } else if (clock64() - t_idle > SB_MBAR_TIMEOUT_CYCLES) {
-        printf("sonar_b200: rel-pos attention MMA issuer stuck block=%d phases=(%d,%d)\n", blockIdx.x, ph0, ph1);
-        __trap();
+        const int j0 = u.kt * 128;
+        const int n0 = S_center - 1 - (u.q0 + 127) + j0;  // p row of window column 0 (may be negative: zero filled)
+        mbar_wait(&bar[KP_EMPTY], (n & 1) ^ 1);
+        mbar_arrive_expect_tx(&bar[KP_FULL], 3 * kTile);
+        tma_load_2d(smem + kOffK, &tm_qkv, &bar[KP_FULL], D + col, u.tok0 + j0);
+        tma_load_2d(smem + kOffPlo, &tm_p, &bar[KP_FULL], col, n0);
+        tma_load_2d(smem + kOffPlo + kTile, &tm_p, &bar[KP_FULL], col, n0 + 128);
+        mbar_wait(&bar[V_EMPTY], (n & 1) ^ 1);
+        mbar_arrive_expect_tx(&bar[V_FULL], kTile);
+        tma_load_2d(smem + kOffV, &tm_qkv, &bar[V_FULL], 2 * D + col, u.tok0 + j0);
+        ++n;
+        u.advance();
       }
     }
-  } else if (warp >= 4) {
-    // ============================ softmax + epilogue: one thread per query row ============================
-    const int g = (warp - 4) >> 2;
-    const int wq = warp & 3;  // TMEM lane quarter = 32-row block of the query tile
-    const int row = wq * 32 + lane;
-    const int shift = 31 - lane;
-    const uint32_t lane_base = uint32_t(wq * 32) << 16;
-    const uint32_t tS = tmem_base + g * 256 + lane_base, tB = tS + 128;
-    uint64_t* bar = bars + g * kNumBars;
+  } else {
+    // ============================ scores, softmax, P.V: 64 query rows per warpgroup ============================
+    const int cwg = wg_idx - 1;
+    const int fr = (warp & 3) * 16 + (lane >> 2);  // fragment rows fr and fr + 8 of this warpgroup's 64
+    const int cq = 2 * (lane & 3);                 // fragment columns 8 j + cq, + 1
+    float* bw = smem_bw + cwg * 64 * kBLd;
+    const uint32_t bar_id = 1 + cwg;
     const float sl2 = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
-    RelStream u;
-    u.init(cu, tile_cu, B, H, blockIdx.x + g * gridDim.x, 2 * gridDim.x);
-    uint32_t n = 0;
-    // Softmax state of the query row across the key tiles of an item.  The exponentials are taken against a REFERENCE m_ref
-    // that is only raised when a score exceeds it by more than kTau (then everything accumulated so far is rescaled): the
-    // probabilities stay below 2^8 relative to the reference, well inside bf16 / fp32 range, and the common case needs no
-    // second pass over the scores and no per-tile rescaling of the accumulator.
-    constexpr float kTau = 8.0f / (0.125f * 1.4426950408889634f);
-    float m_ref = -CUDART_INF_F, l_run = 0.f;
-    float o_acc[64];
+    const uint32_t sbase = smem_u32(smem);
+    float m_run[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_run[2] = {0.f, 0.f};  // l_run: this lane's share of the row sum
+    float o[32];
     while (u.valid) {
       const int kv_valid = min(128, u.len - u.kt * 128);
-      const int nch = (kv_valid + 31) >> 5;  // 32-key chunks holding valid keys
+      const bool active = u.q0 + cwg * 64 < u.len;  // (warpgroup-uniform) this half of the query tile holds queries
+      const bool last = (u.kt == u.nt - 1);
       if (u.kt == 0) {
-        m_ref = -CUDART_INF_F;
-        l_run = 0.f;
-#pragma unroll
-        for (int j = 0; j < 64; ++j) o_acc[j] = 0.f;
+        m_run[0] = m_run[1] = -CUDART_INF_F;
+        l_run[0] = l_run[1] = 0.f;
+        mbar_wait(&bar[Q_FULL], ni & 1);
+        ++ni;
       }
-      float sum = 0.f;       // this key tile's share of the row sum (relative to m_ref)
-      uint32_t done = 0;     // chunks of this tile whose P is already in tensor memory (warp-uniform)
-
-      // sc = the complete scores of chunk c -> probabilities (bf16 pairs) over the chunk's own S columns
-      auto finalize = [&](int c, uint32_t (&sc)[32]) {
-        const int lim = kv_valid - c * 32;
-        if (lim < 32) {  // the chunk reaches past the utterance: those keys get probability exactly 0
+      mbar_wait(&bar[KP_FULL], n & 1);
+      float s[64];
+      if (active) {
+        const uint64_t qu = wgmma_desc_kmajor_sw128(sbase + kOffQu + cwg * 64 * 128);
+        const uint64_t qv = wgmma_desc_kmajor_sw128(sbase + kOffQv + cwg * 64 * 128);
+        const uint64_t kd = wgmma_desc_kmajor_sw128(sbase + kOffK);
+        // Pw rows [64 - 64 cwg + 96 hb, + 96) for half hb of this warpgroup's window
+        const uint32_t pw = sbase + kOffPlo + (64 - 64 * cwg) * 128;
+        float bb[48];
+        // the two Bw halves first and S1 last: at most 64 + 32 accumulator registers are live next to each product
+        wgmma_fence_regs(bb);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 32; ++k)
-            if (k >= lim) sc[k] = __float_as_uint(-CUDART_INF_F);
+        for (int k = 0; k < 4; ++k) wgmma_m64n96k16_ss(bb, qv + uint64_t(2 * k), wgmma_desc_kmajor_sw128(pw) + uint64_t(2 * k), k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(bb);
+        named_bar_sync(bar_id, 128);  // the previous unit's gathers are done
+#pragma unroll
+        for (int j = 0; j < 12; ++j) {
+          float* d = bw + fr * kBLd + 8 * j + cq;
+          d[0] = bb[4 * j]; d[1] = bb[4 * j + 1];
+          d[8 * kBLd] = bb[4 * j + 2]; d[8 * kBLd + 1] = bb[4 * j + 3];
         }
-        float m0 = __uint_as_float(sc[0]), m1 = __uint_as_float(sc[1]);
+        wgmma_fence_regs(bb);
+        wgmma_fence();
 #pragma unroll
-        for (int k = 2; k < 32; k += 2) {
-          m0 = fmaxf(m0, __uint_as_float(sc[k]));
-          m1 = fmaxf(m1, __uint_as_float(sc[k + 1]));
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n96k16_ss(bb, qv + uint64_t(2 * k), wgmma_desc_kmajor_sw128(pw + 96 * 128) + uint64_t(2 * k), k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(bb);
+#pragma unroll
+        for (int j = 0; j < 12; ++j) {
+          float* d = bw + fr * kBLd + 96 + 8 * j + cq;
+          d[0] = bb[4 * j]; d[1] = bb[4 * j + 1];
+          d[8 * kBLd] = bb[4 * j + 2]; d[8 * kBLd + 1] = bb[4 * j + 3];
         }
-        const float cm = fmaxf(m0, m1);
-        const bool bump = cm > m_ref + kTau;  // always on the item's first chunk (m_ref = -inf)
-        if (__any_sync(0xffffffffu, bump)) {   // warp-uniform branch; lanes that keep their reference scale by exactly 1
-          const float m_new = bump ? cm : m_ref;
-          const float f = ex2f((m_ref - m_new) * sl2);
-          l_run *= f;
-          sum *= f;
+        wgmma_fence_regs(s);
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 64; ++j) o_acc[j] *= f;
-          if (done) tmem_st_wait();  // (their tcgen05.st must have landed before they are read back)
-          for (int cc = 0; cc < 4; ++cc) {  // probabilities of this tile already written against the old reference
-            if (!(done & (1u << cc))) continue;
-            uint32_t pk[16];
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                : "=r"(pk[0]), "=r"(pk[1]), "=r"(pk[2]), "=r"(pk[3]), "=r"(pk[4]), "=r"(pk[5]), "=r"(pk[6]), "=r"(pk[7]),
-                  "=r"(pk[8]), "=r"(pk[9]), "=r"(pk[10]), "=r"(pk[11]), "=r"(pk[12]), "=r"(pk[13]), "=r"(pk[14]), "=r"(pk[15])
-                : "r"(tS + cc * 32)
-                : "memory");
-            tmem_ld_wait();
+        for (int k = 0; k < 4; ++k) wgmma_m64n128k16_ss(s, qu + uint64_t(2 * k), kd + uint64_t(2 * k), k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+      }
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&bar[KP_EMPTY]);             // K and Pw are dead
+        if (last) mbar_arrive(&bar[Q_EMPTY]);    // last key tile of the item: Qu, Qv are dead too
+      }
+      uint32_t pa[8][4];
+      float alpha[2] = {1.f, 1.f};
+      if (active) {
+        named_bar_sync(bar_id, 128);  // Bw complete
+        // the shift: query row rl, key jl reads Bw[rl][63 - rl + jl]
+        const float* g0 = bw + fr * kBLd + 63 - fr + cq;
+        const float* g1 = bw + (fr + 8) * kBLd + 63 - (fr + 8) + cq;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162*>(&pk[j]);
-              pk[j] = pack_bf16x2(__low2float(h2) * f, __high2float(h2) * f);
-            }
-            tmem_st_32x16(tS + cc * 32, pk);
+        for (int j = 0; j < 16; ++j) {
+          s[4 * j] += g0[8 * j];
+          s[4 * j + 1] += g0[8 * j + 1];
+          s[4 * j + 2] += g1[8 * j];
+          s[4 * j + 3] += g1[8 * j + 1];
+        }
+        // keys >= kv_valid are beyond the utterance: -inf -> probability exactly 0
+        if (kv_valid < 128) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            if (8 * j + cq >= kv_valid) s[4 * j] = s[4 * j + 2] = -CUDART_INF_F;
+            if (8 * j + cq + 1 >= kv_valid) s[4 * j + 1] = s[4 * j + 3] = -CUDART_INF_F;
           }
-          m_ref = m_new;
         }
-        const float mxs = m_ref * sl2;
-        uint32_t pk[16];
-        float s0 = 0.f, s1 = 0.f;
+        float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
 #pragma unroll
-        for (int k = 0; k < 32; k += 2) {
-          const float p0 = ex2f(fmaf(__uint_as_float(sc[k]), sl2, -mxs));
-          const float p1 = ex2f(fmaf(__uint_as_float(sc[k + 1]), sl2, -mxs));
-          s0 += p0;
-          s1 += p1;
-          pk[k >> 1] = pack_bf16x2(p0, p1);
+        for (int j = 0; j < 16; ++j) {
+          mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
+          mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
         }
-        sum += s0 + s1;
-        tmem_st_32x16(tS + c * 32, pk);  // over the first 16 of the chunk's 32 score columns (its scores are in registers)
-        done |= 1u << c;
-      };
-      // chunk c gets its position terms from window columns [colB, colB + 64) of the resident half of B
-      auto fold = [&](int c, int colB) {
-        uint32_t lo[32], hi[32], sc[32];
-        tmem_ld_32x32(tB + colB, lo);
-        tmem_ld_32x32(tB + colB + 32, hi);
-        tmem_ld_32x32(tS + c * 32, sc);
-        tmem_ld_wait();
-        barrel_shift(lo, hi, shift);
+        float mxs[2];
 #pragma unroll
-        for (int k = 0; k < 32; ++k) sc[k] = __float_as_uint(__uint_as_float(sc[k]) + __uint_as_float(lo[k]));
-        finalize(c, sc);
-      };
-
-      mbar_wait(&bar[AB_FULL], n & 1);
-      tc_fence_after();
-      // ---- pass A: low half of B (window columns 0..127): chunks c < wq complete; the diagonal chunk c == wq needs
-      //      columns 96..127 of this half (kept in registers) and 128..158 of the high half ----
-      for (int c = 0; c < nch && c < wq; ++c) fold(c, 96 - 32 * (wq - c));
-      uint32_t dg[32];
-      const bool has_diag = wq < nch;
-      if (has_diag) {
-        tmem_ld_32x32(tB + 96, dg);
-        tmem_ld_wait();
+        for (int r = 0; r < 2; ++r) {
+          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+          const float m_new = fmaxf(m_run[r], mx[r]);   // finite: key 0 of every tile is valid
+          alpha[r] = ex2f((m_run[r] - m_new) * sl2);     // 0 on the first key tile (m_run = -inf)
+          m_run[r] = m_new;
+          mxs[r] = m_new * sl2;
+        }
+        float sum[2] = {0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float p0 = ex2f(fmaf(s[4 * j], sl2, -mxs[0])), p1 = ex2f(fmaf(s[4 * j + 1], sl2, -mxs[0]));
+          const float p2 = ex2f(fmaf(s[4 * j + 2], sl2, -mxs[1])), p3 = ex2f(fmaf(s[4 * j + 3], sl2, -mxs[1]));
+          sum[0] += p0 + p1;
+          sum[1] += p2 + p3;
+          pa[j >> 1][(j & 1) * 2] = pack_bf16x2(p0, p1);      // A fragment of k-step j / 2: (row, keys) then (row + 8, keys)
+          pa[j >> 1][(j & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+        }
+        l_run[0] = l_run[0] * alpha[0] + sum[0];
+        l_run[1] = l_run[1] * alpha[1] + sum[1];
       }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar[A_DONE]);
-      // ---- pass B: high half of B, now in the same TMEM columns: the diagonal chunk and the chunks c > wq ----
-      mbar_wait(&bar[BHI_FULL], n & 1);
-      tc_fence_after();
-      if (has_diag) {
-        uint32_t hi[32], sc[32];
-        tmem_ld_32x32(tB, hi);
-        tmem_ld_32x32(tS + wq * 32, sc);
-        tmem_ld_wait();
-        barrel_shift(dg, hi, shift);
+      mbar_wait(&bar[V_FULL], n & 1);
+      if (active) {
+        if (u.kt > 0) {
 #pragma unroll
-        for (int k = 0; k < 32; ++k) sc[k] = __float_as_uint(__uint_as_float(sc[k]) + __uint_as_float(dg[k]));
-        finalize(wq, sc);
+          for (int j = 0; j < 8; ++j) {
+            o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
+            o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
+          }
+        }
+        // all 8 k-steps run (a branch around a wgmma would serialize them): masked keys have P = 0 exactly, and the V rows
+        // behind them are other utterances' finite values or TMA zero fill
+        const uint64_t vd = wgmma_desc_mnmajor_sw128(sbase + kOffV);
+        wgmma_fence_regs(o);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          wgmma_m64n64k16_rs_bt(o, pa[k], vd + uint64_t(k * (2048 >> 4)), (u.kt > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
       }
-      for (int c = wq + 1; c < nch; ++c) fold(c, 32 * (c - wq) - 32);
-      l_run += sum;
-      tmem_st_wait();
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bar[P_READY]);
-      // ---- O tile of this key tile (relative to the same reference) -> register accumulator ----
-      mbar_wait(&bar[O_FULL], n & 1);
-      tc_fence_after();
-      uint32_t o[2][32];
-      tmem_ld_32x32(tB, o[0]);
-      tmem_ld_32x32(tB + 32, o[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar[O_FREE]);
+      if (lane == 0) mbar_arrive(&bar[V_EMPTY]);
+      if (active && last) {
 #pragma unroll
-      for (int j = 0; j < 64; ++j) o_acc[j] += __uint_as_float(o[j >> 5][j & 31]);
-      if (u.kt == u.nt - 1 && u.q0 + row < u.len) {
-        const float inv = 1.0f / l_run;
-        uint4* dst = reinterpret_cast<uint4*>(out + (long long)(u.tok0 + u.q0 + row) * D + u.h * 64);
+        for (int r = 0; r < 2; ++r) {
+          float l = l_run[r];
+          l += __shfl_xor_sync(0xffffffffu, l, 1);
+          l += __shfl_xor_sync(0xffffffffu, l, 2);
+          const int qrow = u.q0 + cwg * 64 + fr + 8 * r;
+          if (qrow < u.len) {
+            const float inv = 1.0f / l;
+            uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)(u.tok0 + qrow) * D + u.h * 64 + cq);
 #pragma unroll
-        for (int q = 0; q < 8; ++q)
-          dst[q] = make_uint4(pack_bf16x2(o_acc[8 * q] * inv, o_acc[8 * q + 1] * inv),
-                              pack_bf16x2(o_acc[8 * q + 2] * inv, o_acc[8 * q + 3] * inv),
-                              pack_bf16x2(o_acc[8 * q + 4] * inv, o_acc[8 * q + 5] * inv),
-                              pack_bf16x2(o_acc[8 * q + 6] * inv, o_acc[8 * q + 7] * inv));
+            for (int j = 0; j < 8; ++j) dst[4 * j] = pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
+          }
+        }
       }
       ++n;
       u.advance();
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<1>(tmem_base, 512);
 }
 
 // qu = bf16(q + u), qv = bf16(q + v): q = first D columns of the packed qkv rows; u, v fp32 [D]  (8 elements per thread)
@@ -507,7 +370,7 @@ int attention_relpos_tc(const __nv_bfloat16* qkv, const __nv_bfloat16* p, const 
   if (first_use_on_device(attr_set)) {
     SB_CUDA_CHECK(cudaFuncSetAttribute(attention_relpos_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
   }
-  const int grid = num_sms > 0 ? num_sms : 148;
+  const int grid = num_sms > 0 ? num_sms : device_sm_count();
   attention_relpos_tc_kernel<<<(unsigned)grid, kThreads, kSmemBytes, stream>>>(tm_qu, tm_qv, tm_qkv, tm_p, cu_seqlens, B, H,
                                                                                S_center, out);
   SB_CUDA_CHECK(cudaGetLastError());

@@ -1,4 +1,4 @@
-// tcgen05 self-attention over PACKED variable-length sequences (any length the position table allows).
+// wgmma self-attention over PACKED variable-length sequences (any length the position table allows).
 //
 // Reference semantics: fairseq2 StandardMultiheadAttention + create_default_sdpa
 // (sonar/models/sonar_text/factory.py:130-141) = F.scaled_dot_product_attention with a key-padding mask,
@@ -6,26 +6,20 @@
 // "mask" is simply: keys >= len get probability exactly 0.
 //
 // Work decomposition.  An ITEM is (sentence b, head h).  Its queries are cut into 128-row tiles, its keys into 128-key
-// tiles, and a UNIT is one (query tile, key tile) pair:
-//     S[128 x 128] = Q[128 x 64] . K[128 x 64]^T      4 x tcgen05.mma (M=128, N=128, K=16), operands K-major
-//     P            = exp2((S - m) * scale)            softmax numerators, ONE THREAD PER QUERY ROW reading TMEM
-//     O[128 x 64]  = P[128 x 128] . V[128 x 64]       <= 8 x tcgen05.mma (M=128, N=64, K=16), V is the MN-major B operand
-// For sentences of at most 128 tokens (BASELINE config 2) an item is exactly one unit; longer sentences run
-// nq x nkv units with the usual online-softmax rescaling of a register accumulator between key tiles.
+// tiles, and a UNIT is one (query tile, key tile) pair; each of the two consumer warpgroups owns 64 query rows of it:
+//     S[64 x 128] = Q[64 x 64] . K[128 x 64]^T       4 x wgmma.m64n128k16, operands K-major in shared memory
+//     P           = exp2((S - m) * scale)            softmax numerators on the accumulator fragments (a row = 4 lanes)
+//     O[64 x 64] += P[64 x 128] . V[128 x 64]        <= 8 x wgmma.m64n64k16, A = P from REGISTERS, V the MN-major B operand
+// For sentences of at most 128 tokens an item is exactly one unit; longer sentences run nq x nkv units with the usual
+// online-softmax rescaling of the register accumulator between key tiles.
 //
-// One persistent CTA per SM, warp-specialised, everything asynchronous:
-//   warp 0   TMA producer: [128 x 64] bf16 tiles (SWIZZLE_128B) of the next units into two rings -- Q|K pairs (3 stages,
-//            released as soon as S = Q K^T has retired) and V tiles (6 stages, released when P.V has retired) -- so loads
-//            run 3 units ahead of the S products and 6 ahead of the P.V products: the op is HBM-bound (reads 6 B, writes
-//            2 B per token and dim; 1.2 % of the encoder FLOPs) and what matters is bytes in flight per SM
-//   warp 1   MMA issuer (one elected lane): S for unit u, then P.V for unit u-1, so the tensor core always has the other
-//            softmax group's S queued while one group is busy with exponentials
-//   warp 2   TMEM allocator (512 columns: S0 | S1 | O0 | O1 | P0 | P1)
-//   warps 4-7 / 8-11   two softmax + epilogue warpgroups (TMEM lane quarter = warp % 4); group g owns the items with
-//            g = local item index & 1 and the TMEM buffers S[g], O[g], P[g]
-// The softmax is two-pass over TMEM (row maximum, then exponentials), 32 columns at a time, so a thread never holds more
-// than one chunk of the score row.  P never touches shared memory: the bf16 probabilities go back to TENSOR MEMORY
-// (tcgen05.st, two per 32-bit column) and P.V reads its A operand from there (tcgen05.mma with A in TMEM).
+// One persistent CTA per SM, warp-specialised:
+//   warpgroup 0    TMA producer (one thread): [128 x 64] bf16 tiles (SWIZZLE_128B) of the next units into two rings -- Q|K
+//                  pairs (3 stages, released as soon as S = Q K^T has retired) and V tiles (6 stages, released when P.V has
+//                  retired): the op is HBM-bound (reads 6 B, writes 2 B per token and dim; 1.2 % of the encoder FLOPs) and
+//                  what matters is bytes in flight per SM
+//   warpgroups 1-2 S, softmax, P.V and the output rows of their 64 queries.  P never touches shared memory: the
+//                  accumulator layout of S is the A-operand register layout of P.V.
 
 #include "common.cuh"
 #include "sonar_b200_internal.h"
@@ -42,17 +36,8 @@ constexpr int kRingBytes = kQkStages * 2 * kTile + kVStages * kTile;  // 192 KB
 constexpr int kBarBytes = 512;
 constexpr int kCuSmemInts = 8192;  // cu_seqlens is staged in shared memory when the batch has < 8192 sentences
 constexpr int kSmemBytes = kRingBytes + kBarBytes + kCuSmemInts * 4 + 1024;  // + alignment slack
-// TMEM columns: S[g] = g * 128 (fp32 scores), O[g] = 256 + g * 64 (fp32), P[g] = 384 + g * 64 (bf16 pairs)
-constexpr uint32_t kTmemO = 256, kTmemP = 384;
+static_assert(kSmemBytes <= 232448, "shared memory budget of one sm_90 block");
 constexpr int kThreads = 384;
-
-// MN-major B operand (V: rows = keys (K dim), 64 contiguous head dims = one 128 B swizzle row):
-// 8-key groups are 1024 B apart (SBO); a single 64-wide atom along MN, LBO = 128 keys * 128 B.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr) {
-  uint64_t lo = ((smem_addr >> 4) & 0x3FFFu) | (uint64_t((128u * 128u) >> 4) << 16);
-  uint64_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-  return lo | (hi << 32);
-}
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -60,8 +45,8 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-// The unit sequence of one softmax group inside this CTA: items blockIdx.x + (2*i + g) * gridDim.x, i = 0, 1, ...,
-// each expanded into its (query tile, key tile) units.  Every warp role walks identical copies.
+// The unit sequence of this CTA: items blockIdx.x + i * gridDim.x, i = 0, 1, ..., each expanded into its
+// (query tile, key tile) units.  Every warp role walks identical copies.
 struct UnitStream {
   const int32_t* cu;
   int H, num_items, item, stride;
@@ -105,17 +90,13 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, const int32_t* c
   uint8_t* smem_v = smem + kQkStages * 2 * kTile;       // [kVStages]
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes);
   uint64_t* full_qk = bars;                       // [kQkStages] TMA: Q and K landed
-  uint64_t* empty_qk = full_qk + kQkStages;       // [kQkStages] MMA: S retired -> the Q | K pair is free
+  uint64_t* empty_qk = full_qk + kQkStages;       // [kQkStages] S retired in every consumer warp -> the Q | K pair is free
   uint64_t* full_v = empty_qk + kQkStages;        // [kVStages] TMA: V landed
-  uint64_t* empty_v = full_v + kVStages;          // [kVStages] MMA: P.V retired -> the V tile is free
-  uint64_t* s_full = empty_v + kVStages;          // [2] MMA: S[g] complete
-  uint64_t* p_ready = s_full + 2;                 // [2] softmax group g: P[g] written and S[g] fully read (4 warp arrivals)
-  uint64_t* o_full = s_full + 4;                  // [2] MMA: O[g] complete (P[g] consumed)
-  uint64_t* o_free = s_full + 6;                  // [2] group g: O[g] read out of TMEM (4 warp arrivals)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(s_full + 8);
+  uint64_t* empty_v = full_v + kVStages;          // [kVStages] P.V retired in every consumer warp -> the V tile is free
   int32_t* cu_smem = reinterpret_cast<int32_t*>(smem + kRingBytes + kBarBytes);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg_idx = threadIdx.x >> 7;
   const int D = H * 64;
   const int num_items = B * H;
   // every role looks sentence boundaries up once per item: keep them in shared memory (one LDS instead of an L2 round trip)
@@ -124,44 +105,31 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, const int32_t* c
     for (int i = threadIdx.x; i <= B; i += kThreads) cu_smem[i] = cu_g[i];
     cu = cu_smem;
   }
-
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_qkv);
     for (int i = 0; i < kQkStages; ++i) {
       mbar_init(&full_qk[i], 1);
-      mbar_init(&empty_qk[i], 1);
+      mbar_init(&empty_qk[i], 8);
     }
     for (int i = 0; i < kVStages; ++i) {
       mbar_init(&full_v[i], 1);
-      mbar_init(&empty_v[i], 1);
-    }
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(&s_full[g], 1);
-      mbar_init(&p_ready[g], 4);
-      mbar_init(&o_full[g], 1);
-      mbar_init(&o_free[g], 4);
+      mbar_init(&empty_v[i], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<1>(tmem_ptr_smem, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  UnitStream u;
+  u.init(cu, H, num_items, blockIdx.x, gridDim.x);
+  int sq = 0, sv = 0;
+  uint32_t phq = 0, phv = 0;
+
+  if (wg_idx == 0) {
     // ============================ TMA producer ============================
-    if (lane == 0) {
-      UnitStream s0, s1;  // (two named streams, selected by value: indexing an array of them would put them in local memory)
-      s0.init(cu, H, num_items, blockIdx.x, 2 * gridDim.x);
-      s1.init(cu, H, num_items, blockIdx.x + gridDim.x, 2 * gridDim.x);
-      int sq = 0, sv = 0;
-      uint32_t phq = 0, phv = 0;
-      for (int turn = 0; s0.valid || s1.valid; ++turn) {
-        const bool g1 = (turn & 1) ? s1.valid : !s0.valid;
-        const int col = (g1 ? s1.h : s0.h) * 64;
-        const int qrow = g1 ? s1.tok0 + s1.qt * 128 : s0.tok0 + s0.qt * 128;
-        const int krow = g1 ? s1.tok0 + s1.kt * 128 : s0.tok0 + s0.kt * 128;
+    if (warp == 0 && lane == 0) {
+      while (u.valid) {
+        const int col = u.h * 64;
+        const int qrow = u.tok0 + u.qt * 128, krow = u.tok0 + u.kt * 128;
         uint8_t* qk = smem_qk + sq * 2 * kTile;
         mbar_wait(&empty_qk[sq], phq ^ 1);
         mbar_arrive_expect_tx(&full_qk[sq], 2 * kTile);
@@ -170,209 +138,123 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, const int32_t* c
         mbar_wait(&empty_v[sv], phv ^ 1);
         mbar_arrive_expect_tx(&full_v[sv], kTile);
         tma_load_2d(smem_v + sv * kTile, &tm_qkv, &full_v[sv], 2 * D + col, krow);
-        if (g1) s1.advance(); else s0.advance();
+        u.advance();
         if (++sq == kQkStages) { sq = 0; phq ^= 1; }
         if (++sv == kVStages) { sv = 0; phv ^= 1; }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ============================ MMA issuer ============================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16_f32(128, 128);
-      constexpr uint32_t idesc_o = umma_idesc_bf16_f32(128, 64) | (1u << 16);  // B operand MN-major
-      UnitStream s0, s1;
-      s0.init(cu, H, num_items, blockIdx.x, 2 * gridDim.x);
-      s1.init(cu, H, num_items, blockIdx.x + gridDim.x, 2 * gridDim.x);
-      int sq = 0, sv = 0;
-      uint32_t phq = 0, phv = 0;
-      uint32_t n0 = 0, n1 = 0;  // units issued per group
-      // the unit whose P.V is still to be issued (one behind the S issue)
-      int pend_g = -1, pend_sv = 0, pend_ksteps = 0;
-      uint32_t pend_phv = 0, pend_n = 0;
-      auto issue_pv = [&]() {
-        const int g = pend_g;
-        mbar_wait(&p_ready[g], pend_n & 1);             // P[g] in tensor memory, S[g] read
-        mbar_wait(&full_v[pend_sv], pend_phv);
-        if (pend_n > 0) mbar_wait(&o_free[g], (pend_n - 1) & 1);  // the group's previous O has been read out
-        tc_fence_after();
-        const uint32_t tmem_o = tmem_base + kTmemO + g * 64;
-        const uint32_t tmem_p = tmem_base + kTmemP + g * 64;
-        const uint32_t v_addr = smem_u32(smem_v + pend_sv * kTile);
-        for (int k = 0; k < pend_ksteps; ++k) {  // 16 keys per k-step: 8 TMEM columns of P, 16 rows (2 KB) of V
-          const uint64_t vd = umma_desc_mnmajor_sw128(v_addr + k * 2048);
-          umma_bf16_ts(tmem_o, tmem_p + 8 * k, vd, idesc_o, k != 0);
-        }
-        umma_commit<1>(&o_full[g]);
-        umma_commit<1>(&empty_v[pend_sv]);
-        pend_g = -1;
-      };
-      for (int turn = 0; s0.valid || s1.valid; ++turn) {
-        const bool g1 = (turn & 1) ? s1.valid : !s0.valid;
-        const int g = g1 ? 1 : 0;
-        const uint32_t ng = g1 ? n1 : n0;
-        const int kv_valid = g1 ? min(128, s1.len - s1.kt * 128) : min(128, s0.len - s0.kt * 128);
-        uint8_t* base = smem_qk + sq * 2 * kTile;
-        // a P that is already waiting goes to the tensor core before this thread blocks on the next unit's loads
-        if (pend_g >= 0 && mbar_test_wait(&p_ready[pend_g], pend_n & 1)) issue_pv();
-        // ---- S = Q K^T for this unit ----
-        mbar_wait(&full_qk[sq], phq);
-        if (ng > 0) {
-          if (pend_g == g) issue_pv();                 // same group twice in a row: its P.V must go first
-          mbar_wait(&p_ready[g], (ng - 1) & 1);        // S[g] of the group's previous unit has been read
-        }
-        tc_fence_after();
-        {
-          const uint64_t qd = umma_desc_kmajor_sw128(smem_u32(base));
-          const uint64_t kd = umma_desc_kmajor_sw128(smem_u32(base + kTile));
-          const uint32_t tmem_s = tmem_base + g * 128;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16<1>(tmem_s, qd + uint64_t(2 * k), kd + uint64_t(2 * k), idesc_s, k != 0);
-          umma_commit<1>(&s_full[g]);
-          umma_commit<1>(&empty_qk[sq]);  // Q and K are dead once S has retired: their slot goes straight back to the producer
-        }
-        // ---- P.V of the previous unit (normally the other group's) ----
-        if (pend_g >= 0) issue_pv();
-        pend_g = g;
-        pend_sv = sv;
-        pend_phv = phv;
-        pend_ksteps = (kv_valid + 15) >> 4;
-        pend_n = ng;
-        if (g1) { ++n1; s1.advance(); } else { ++n0; s0.advance(); }
-        if (++sq == kQkStages) { sq = 0; phq ^= 1; }
-        if (++sv == kVStages) { sv = 0; phv ^= 1; }
-      }
-      if (pend_g >= 0) issue_pv();
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ============================ softmax + epilogue: one thread per query row ============================
-    const int g = (warp - 4) >> 2;
-    const int wq = warp & 3;  // TMEM lane quarter
-    const int row = wq * 32 + lane;
-    const uint32_t lane_base = uint32_t(wq * 32) << 16;
-    const uint32_t tmem_s = tmem_base + g * 128 + lane_base;
-    const uint32_t tmem_o = tmem_base + kTmemO + g * 64 + lane_base;
-    const uint32_t tmem_p = tmem_base + kTmemP + g * 64 + lane_base;
-    const float sl2 = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
-    UnitStream u;
-    u.init(cu, H, num_items, blockIdx.x + g * gridDim.x, 2 * gridDim.x);
-    uint32_t n = 0;
-    float m_run = -CUDART_INF_F, l_run = 0.f;
-    float o_acc[64];
+  } else {
+    // ============================ S, softmax, P.V: 64 query rows per warpgroup, a row = the 4 lanes of a quad ============
+    const int cwg = wg_idx - 1;
+    const int r_lo = cwg * 64 + (warp & 3) * 16 + (lane >> 2);  // query rows r_lo and r_lo + 8 of the tile
+    const int cq = 2 * (lane & 3);                              // fragment columns 8 j + cq, + 1
+    const float sl2 = 0.125f * 1.4426950408889634f;             // 1/sqrt(64) * log2(e)
+    float m_run[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_run[2] = {0.f, 0.f};  // l_run: this lane's share of the row sum
+    float o[32];
     while (u.valid) {
       const int kv_valid = min(128, u.len - u.kt * 128);
-      const int nch = (kv_valid + 31) >> 5;  // 32-key chunks holding valid keys
-      const bool single = (u.nt == 1);
-      if (u.kt == 0) { m_run = -CUDART_INF_F; l_run = 0.f; }
-
-      mbar_wait(&s_full[g], n & 1);
-      tc_fence_after();
-      // ---- pass 1: row maximum over the valid keys ----
-      float mx = -CUDART_INF_F;
-      for (int c = 0; c < nch; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_s + c * 32, v);
-        tmem_ld_wait();
-        const int lim = kv_valid - c * 32;  // keys >= lim of this chunk are beyond the sentence
-        if (lim < 32) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (j >= lim) v[j] = __float_as_uint(-CUDART_INF_F);
-        }
-        float m0 = __uint_as_float(v[0]), m1 = __uint_as_float(v[1]);
-#pragma unroll
-        for (int j = 2; j < 32; j += 2) {
-          m0 = fmaxf(m0, __uint_as_float(v[j]));
-          m1 = fmaxf(m1, __uint_as_float(v[j + 1]));
-        }
-        mx = fmaxf(mx, fmaxf(m0, m1));
-      }
-      const float m_new = fmaxf(m_run, mx);
-      const float alpha = fast_exp2((m_run - m_new) * sl2);  // 0 on the first key tile (m_run = -inf)
-      const float mxs = m_new * sl2;
-      // ---- pass 2: p = exp2(s*c - m*c), row sum, bf16 pairs -> tensor memory (the A operand of P.V) ----
-      float sum0 = 0.f, sum1 = 0.f;
-      for (int c = 0; c < nch; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_s + c * 32, v);
-        tmem_ld_wait();
-        const int lim = kv_valid - c * 32;
-        if (lim < 32) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (j >= lim) v[j] = __float_as_uint(-CUDART_INF_F);  // -inf -> probability exactly 0
-        }
-        uint32_t pk[16];
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          const float p0 = fast_exp2(fmaf(__uint_as_float(v[j]), sl2, -mxs));
-          const float p1 = fast_exp2(fmaf(__uint_as_float(v[j + 1]), sl2, -mxs));
-          sum0 += p0;
-          sum1 += p1;
-          pk[j >> 1] = pack_bf16x2(p0, p1);  // key j in the low half: K runs along the column, two keys per column
-        }
-        tmem_st_32x16(tmem_p + c * 16, pk);
-      }
-      // P.V consumes whole 16-key k-steps and every written 32-key chunk is complete (masked keys as zeros)
-      l_run = l_run * alpha + (sum0 + sum1);
-      m_run = m_new;
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_ready[g]);
-      // ---- O tile: accumulate / write out ----
-      mbar_wait(&o_full[g], n & 1);
-      tc_fence_after();
-      uint32_t o[2][32];
-      tmem_ld_32x32(tmem_o, o[0]);
-      tmem_ld_32x32(tmem_o + 32, o[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&o_free[g]);
+      const bool active = u.qt * 128 + cwg * 64 < u.len;  // (warpgroup-uniform) this half of the query tile holds queries
       const bool last = (u.kt == u.nt - 1);
-      const int qrow = u.qt * 128 + row;
-      if (single) {
-        if (qrow < u.len) {
-          const float inv = 1.0f / l_run;
-          uint4* dst = reinterpret_cast<uint4*>(out + (long long)(u.tok0 + qrow) * D + u.h * 64);
+      if (u.kt == 0) { m_run[0] = m_run[1] = -CUDART_INF_F; l_run[0] = l_run[1] = 0.f; }
+      float s[64];
+      mbar_wait(&full_qk[sq], phq);
+      if (active) {
+        const uint8_t* base = smem_qk + sq * 2 * kTile;
+        const uint64_t qd = wgmma_desc_kmajor_sw128(smem_u32(base) + cwg * 64 * 128);
+        const uint64_t kd = wgmma_desc_kmajor_sw128(smem_u32(base + kTile));
+        wgmma_fence_regs(s);
+        wgmma_fence();
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const uint32_t* s = &o[q >> 2][(q & 3) * 8];
-            dst[q] = make_uint4(pack_bf16x2(__uint_as_float(s[0]) * inv, __uint_as_float(s[1]) * inv),
-                                pack_bf16x2(__uint_as_float(s[2]) * inv, __uint_as_float(s[3]) * inv),
-                                pack_bf16x2(__uint_as_float(s[4]) * inv, __uint_as_float(s[5]) * inv),
-                                pack_bf16x2(__uint_as_float(s[6]) * inv, __uint_as_float(s[7]) * inv));
+        for (int k = 0; k < 4; ++k) wgmma_m64n128k16_ss(s, qd + uint64_t(2 * k), kd + uint64_t(2 * k), k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_qk[sq]);  // Q and K are dead once S has retired
+      uint32_t pa[8][4];
+      float alpha[2] = {1.f, 1.f};
+      if (active) {
+        // keys >= kv_valid are beyond the sentence: -inf -> probability exactly 0
+        if (kv_valid < 128) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            if (8 * j + cq >= kv_valid) s[4 * j] = s[4 * j + 2] = -CUDART_INF_F;
+            if (8 * j + cq + 1 >= kv_valid) s[4 * j + 1] = s[4 * j + 3] = -CUDART_INF_F;
           }
         }
-      } else {
-        if (u.kt == 0) {
+        float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
 #pragma unroll
-          for (int j = 0; j < 64; ++j) o_acc[j] = __uint_as_float(o[j >> 5][j & 31]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 64; ++j) o_acc[j] = fmaf(o_acc[j], alpha, __uint_as_float(o[j >> 5][j & 31]));
+        for (int j = 0; j < 16; ++j) {
+          mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
+          mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
         }
-        if (last && qrow < u.len) {
-          const float inv = 1.0f / l_run;
-          uint4* dst = reinterpret_cast<uint4*>(out + (long long)(u.tok0 + qrow) * D + u.h * 64);
+        float mxs[2];
 #pragma unroll
-          for (int q = 0; q < 8; ++q)
-            dst[q] = make_uint4(pack_bf16x2(o_acc[8 * q] * inv, o_acc[8 * q + 1] * inv),
-                                pack_bf16x2(o_acc[8 * q + 2] * inv, o_acc[8 * q + 3] * inv),
-                                pack_bf16x2(o_acc[8 * q + 4] * inv, o_acc[8 * q + 5] * inv),
-                                pack_bf16x2(o_acc[8 * q + 6] * inv, o_acc[8 * q + 7] * inv));
+        for (int r = 0; r < 2; ++r) {
+          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+          const float m_new = fmaxf(m_run[r], mx[r]);       // finite: key 0 of every tile is valid
+          alpha[r] = fast_exp2((m_run[r] - m_new) * sl2);    // 0 on the first key tile (m_run = -inf)
+          m_run[r] = m_new;
+          mxs[r] = m_new * sl2;
+        }
+        float sum[2] = {0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float p0 = fast_exp2(fmaf(s[4 * j], sl2, -mxs[0])), p1 = fast_exp2(fmaf(s[4 * j + 1], sl2, -mxs[0]));
+          const float p2 = fast_exp2(fmaf(s[4 * j + 2], sl2, -mxs[1])), p3 = fast_exp2(fmaf(s[4 * j + 3], sl2, -mxs[1]));
+          sum[0] += p0 + p1;
+          sum[1] += p2 + p3;
+          pa[j >> 1][(j & 1) * 2] = pack_bf16x2(p0, p1);      // A fragment of k-step j / 2: (row, keys) then (row + 8, keys)
+          pa[j >> 1][(j & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+        }
+        l_run[0] = l_run[0] * alpha[0] + sum[0];
+        l_run[1] = l_run[1] * alpha[1] + sum[1];
+      }
+      mbar_wait(&full_v[sv], phv);
+      if (active) {
+        if (u.kt > 0) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
+            o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
+          }
+        }
+        // all 8 k-steps run (a branch around a wgmma would serialize them): masked keys have P = 0 exactly, and the V rows
+        // behind them are other sentences' finite values or TMA zero fill
+        const uint64_t vd = wgmma_desc_mnmajor_sw128(smem_u32(smem_v + sv * kTile));
+        wgmma_fence_regs(o);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          wgmma_m64n64k16_rs_bt(o, pa[k], vd + uint64_t(k * (2048 >> 4)), (u.kt > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_v[sv]);
+      if (active && last) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          float l = l_run[r];
+          l += __shfl_xor_sync(0xffffffffu, l, 1);
+          l += __shfl_xor_sync(0xffffffffu, l, 2);
+          const int qrow = u.qt * 128 + r_lo + 8 * r;
+          if (qrow < u.len) {
+            const float inv = 1.0f / l;
+            uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)(u.tok0 + qrow) * D + u.h * 64 + cq);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) dst[4 * j] = pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
+          }
         }
       }
-      ++n;
       u.advance();
+      if (++sq == kQkStages) { sq = 0; phq ^= 1; }
+      if (++sv == kVStages) { sv = 0; phv ^= 1; }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<1>(tmem_base, 512);
 }
 
 }  // namespace
@@ -388,7 +270,7 @@ int attention_packed_tc(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int
     SB_CUDA_CHECK(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
   }
   long long items = (long long)B * H;
-  long long grid = (num_sms > 0 ? num_sms : 148);
+  long long grid = (num_sms > 0 ? num_sms : device_sm_count());
   if (grid > items) grid = items;
   attention_tc_kernel<<<(unsigned)grid, kThreads, kSmemBytes, stream>>>(tm, cu_seqlens, B, H, out);
   SB_CUDA_CHECK(cudaGetLastError());

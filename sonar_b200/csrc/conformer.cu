@@ -1,10 +1,10 @@
-// SONAR speech encoder on sm_100a (BASELINE.json config 3; SURVEY §8 rows a11/a12, App. B.2/B.3):
+// SONAR speech encoder on sm_90a (BASELINE.json config 3; SURVEY §8 rows a11/a12, App. B.2/B.3):
 //   w2v-BERT frontend (stack 2 fbank frames -> LN(160) -> Linear 160->1024)
 //   -> 24 Conformer blocks -> model.layer_norm -> attention pooler (1 BOS query, POST-LN decoder layers) -> [B,1024]
 // following SonarSpeechEncoderModel.forward (sonar/models/sonar_speech/model.py:59-77), factory.py:53-152,
 // nn/encoder_pooler.py:70-83; parameter names per sonar_speech/handler.py:63-100.
 //
-// Every Linear / pointwise conv is the tcgen05 GEMM of gemm_tcgen05.cu (SiLU / ReLU / bias / x += epilogues; the
+// Every Linear / pointwise conv is the wgmma GEMM of gemm_wgmma.cu (SiLU / ReLU / bias / x += epilogues; the
 // macaron 0.5 is folded into the FFN output weights on the host, BatchNorm is folded to scale+shift).  Tokens are
 // PACKED (row = cu[b] + t), so padded positions never exist: the reference zeroes them before the depthwise conv and
 // masks them in the softmax; here they are simply out of range.
@@ -413,16 +413,9 @@ attention_relpos_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid
 // conv module middle: GLU -> depthwise conv (k taps, "same", zero outside the utterance) -> BN(scale,shift) -> SiLU
 //   g bf16 [T, 2D] (pointwise_conv1 output: value | gate), out bf16 [T, D]
 // ---------------------------------------------------------------------------------------------
-// Two adjacent channels per thread: value pairs come out of shared memory as 64-bit loads and every tap is ONE packed
-// fma.rn.f32x2 (FFMA2) for both channels -- the kernel is issue-bound (31 taps per output next to the GLU, BatchNorm and SiLU
-// arithmetic), and the packed form halves the FMA issue slots.  Per output the taps are applied in the order k = 0..KS-1
-// with IEEE fma, exactly as a scalar loop would.
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra = *reinterpret_cast<unsigned long long*>(&a), rb = *reinterpret_cast<unsigned long long*>(&b),
-                     rc = *reinterpret_cast<unsigned long long*>(&c), rd;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  return *reinterpret_cast<float2*>(&rd);
-}
+// Two adjacent channels per thread: value pairs come out of shared memory as 64-bit loads.  Per output the taps are applied
+// in the order k = 0..KS-1 with IEEE fma, one fma per channel (Hopper has no packed fp32 FMA).
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 template <int KS>
 __global__ void __launch_bounds__(128, 5)
@@ -619,7 +612,7 @@ SpWs carve_sp(const SbSpeechEncoder* e, int B, long long T, int smax, void* base
   w.big = reinterpret_cast<__nv_bfloat16*>(take(t * wide * 2));
   w.p = reinterpret_cast<__nv_bfloat16*>(take(np * D * 2));
   w.vp = reinterpret_cast<float*>(take(H * np * 4));
-  w.qu = reinterpret_cast<__nv_bfloat16*>(take(t * D * 2));  // bf16(q + u), bf16(q + v): A operands of the tcgen05 attention
+  w.qu = reinterpret_cast<__nv_bfloat16*>(take(t * D * 2));  // bf16(q + u), bf16(q + v): A operands of the wgmma attention
   w.qv = reinterpret_cast<__nv_bfloat16*>(take(t * D * 2));
   w.e = reinterpret_cast<__nv_bfloat16*>(take(t * D * 2));
   w.px = reinterpret_cast<float*>(take((size_t)B * D * 4));
@@ -657,7 +650,7 @@ int sb_speech_encoder_create(const SbSpeechConfig* cfg, const SbSpeechWeights* w
   SB_CUDA_CHECK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   SB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) { set_last_error("sb_speech_encoder_create: needs a B200-class GPU"); return SB_ERR_CUDA; }
+  if (prop.major != 9) { set_last_error("sb_speech_encoder_create: needs a Hopper H100-class GPU (sm_90)"); return SB_ERR_CUDA; }
   SbSpeechEncoder* e = new (std::nothrow) SbSpeechEncoder();
   if (!e) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   e->cfg = *cfg;
@@ -765,7 +758,7 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
       attention_relpos_kernel<<<dim3((unsigned)((smax + 127) / 128), (unsigned)H, (unsigned)B), kRpThreads, kRpSmem, stream>>>(
           tm_qkv, tm_p, cu_dev, H, L.u_bias, w.vp, Npad, smax, w.h);
       SB_CUDA_CHECK(cudaGetLastError());
-    } else {  // tcgen05 (attention_relpos_tc.cu)
+    } else {  // wgmma (attention_relpos_tc.cu)
       if ((rc = attention_relpos_tc(w.big, w.p, L.u_bias, L.v_bias, cu_dev, B, H, T, Npad, smax, w.qu, w.qv, w.h, e->num_sms,
                                     stream)))
         return rc;

@@ -12,10 +12,10 @@
 //
 // Per step (R = sentences x beam rows, all at the same position t):
 //   x = E[token] * sqrt(d) + pos[t]
-//   24 x { h = LN(x); qkv = h Wqkv^T (tcgen05 GEMM); K/V appended to the cache; attention over positions 0..t
+//   24 x { h = LN(x); qkv = h Wqkv^T (wgmma GEMM); K/V appended to the cache; attention over positions 0..t
 //          through a per-row ancestry table (beam reordering never moves the cache); x += o Wo^T + bo (TMA reduce-add);
 //          x += c_l[sentence]; h = LN(x); x += W2 relu(W1 h + b1) + b2 }
-//   h = LN_final(x);  logits = h E^T  -- never materialised: the tcgen05 GEMM's sweep epilogue keeps a running
+//   h = LN_final(x);  logits = h E^T  -- never materialised: the wgmma GEMM's sweep epilogue keeps a running
 //   top-16 and an online log-sum-exp per row over all 256 206 columns; a merge kernel turns the per-chunk partials
 //   into the 16 best (log-prob, token) pairs per row plus log P(EOS).
 
@@ -429,8 +429,8 @@ int sb_decoder_create(const SbDecoderConfig* cfg, const SbDecoderWeights* w, SbD
   SB_CUDA_CHECK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   SB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) {
-    set_last_error("sb_decoder_create: sm_100a kernels need a B200-class GPU (found sm_%d%d)", prop.major, prop.minor);
+  if (prop.major != 9) {
+    set_last_error("sb_decoder_create: sm_90a kernels need a Hopper H100-class GPU (found sm_%d%d)", prop.major, prop.minor);
     return SB_ERR_CUDA;
   }
   SbDecoder* d = new (std::nothrow) SbDecoder();

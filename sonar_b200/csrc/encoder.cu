@@ -14,7 +14,7 @@
 //
 // Schedule with cfg.ln_fold = 1, 5 launches per layer, no LayerNorm kernel:
 //   embed -> x, h = bf16(x), row stats
-//   24 x [ QKV GEMM (folds LN1: stats + gamma/beta prepared into W', c, b') -> attention (tcgen05) ->
+//   24 x [ QKV GEMM (folds LN1: stats + gamma/beta prepared into W', c, b') -> attention (wgmma) ->
 //          out-proj GEMM (+residual; emits x, bf16(x), stats) -> FFN1 GEMM (folds LN2, +ReLU) ->
 //          FFN2 GEMM (+residual; emits x, bf16(x), stats) ] -> final LN + pool
 // cfg.ln_fold = 0 (what the Python wrapper selects by default: measured faster, see bench.py `ab_layernorm_schedule`) keeps
@@ -156,8 +156,8 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
   SB_CUDA_CHECK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   SB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) {
-    set_last_error("sb_encoder_create: sm_100a kernels need a Blackwell B200-class GPU (found sm_%d%d)", prop.major,
+  if (prop.major != 9) {
+    set_last_error("sb_encoder_create: sm_90a kernels need a Hopper H100-class GPU (found sm_%d%d)", prop.major,
                    prop.minor);
     return SB_ERR_CUDA;
   }

@@ -1,8 +1,8 @@
 // Skinny GEMM for a handful of rows (M <= 64): C[M,N] = epi(A[M,K] . W[N,K]^T + bias).
 //
 // The decoder's beam step at the pipelines' default batch (5 sentences x beam 5 = 25 hypothesis rows) and the speech
-// pooler's single-query layers multiply a few activation rows with full weight matrices.  The 128 x 256 tcgen05 tiles of
-// gemm_tcgen05.cu spend a whole tile's MMA time on mostly-zero rows and put only N/256 CTA pairs on the machine, so a
+// pooler's single-query layers multiply a few activation rows with full weight matrices.  The 128 x 256 wgmma tiles of
+// gemm_wgmma.cu spend a whole tile's MMA time on mostly-zero rows and put only N/256 CTA pairs on the machine, so a
 // [25 x 8192] . [8192 x 1024] product takes ~50 us.  This path is the opposite design point: the work is streaming W once
 // from HBM, so every CTA owns 8 rows of W (one n8 tile -> N/8 CTAs cover the SMs), its 8 warps split K, each lane pulls
 // 16 contiguous bytes of "its" W row and of the activation rows straight from global memory, and the products run on
@@ -131,7 +131,7 @@ gemm_skinny_kernel(const __nv_bfloat16* __restrict__ A, long long lda, const __n
     if (epi == EPI_BIAS_SILU) v = silu_fast(v);
     OutT* dst = C + (long long)r * ldc + n0 + c;
     if constexpr (sizeof(OutT) == 4) {
-      if (epi == EPI_BIAS_RESIDUAL || epi == EPI_BIAS_ACCUM) v = *dst + v;  // same rounding as the tcgen05 path: fl(x + fl(acc + bias))
+      if (epi == EPI_BIAS_RESIDUAL || epi == EPI_BIAS_ACCUM) v = *dst + v;  // same rounding as the wgmma path: fl(x + fl(acc + bias))
       *dst = v;
     } else {
       *dst = __float2bfloat16_rn(v);

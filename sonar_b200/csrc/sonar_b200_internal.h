@@ -38,7 +38,7 @@ inline bool first_use_on_device(bool (&flags)[64]) {
 // so the GEMM that CONSUMES a LayerNorm runs on the un-normalised bf16 copy of the residual stream and applies the
 // per-row (mean, rstd) in its epilogue (`stats_in`, `colsum`), and the GEMM that PRODUCES the residual stream
 // (EPI_BIAS_RESIDUAL_STATS) emits, next to x, that bf16 copy (`h_out`) and per-row partial statistics (`stats_out`):
-// one (mean, M2) pair per kLnPartCols columns of the row (each epilogue warpgroup's share of a 256-column tile), merged by
+// one (mean, M2) pair per kLnPartCols columns of the row (one column half of a 256-column tile), merged by
 // the consumer with Chan's formula (no E[x^2]-mean^2 cancellation).  Saves the LayerNorm kernel's read of x and one of
 // the two passes over h per LayerNorm.
 constexpr int kLnPartCols = 128;
@@ -51,6 +51,14 @@ struct LnFold {
   long long ldh = 0;
   float* stats_out = nullptr;       // producer: [M, N / kLnPartCols, 2]
 };
+
+// SM count of the current device (what `num_sms = 0` means everywhere); 1 if the query fails, so a grid is never empty
+inline int device_sm_count() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1)
+    return 1;
+  return n;
+}
 
 struct GemmArgs {
   const __nv_bfloat16* A;  // [M,K] row-major, ld = lda
@@ -66,14 +74,13 @@ struct GemmArgs {
   int M, N, K;
   int epi;        // EpiMode
   int cta_group;  // 1 or 2
-  int num_sms;    // 0 -> 148
+  int num_sms;    // 0 -> device_sm_count()
   LnFold lf;      // LayerNorm folding (see above); default = off
-  // Opt-in to the weight-streaming path for M <= 64 (gemm_skinny.cu).  It sums K in a different order than the tcgen05
+  // Opt-in to the weight-streaming path for M <= 64 (gemm_skinny.cu).  It sums K in a different order than the wgmma
   // tiles, so a caller that promises results independent of the batch size across the M = 64 boundary (the text
   // encoder: bitwise batch-composition invariance) leaves it off; the decoder step and the speech pooler turn it on.
   int allow_skinny = 0;
-  // 2 (default) = two epilogue warpgroups / 5 mainloop stages; 1 = one epilogue warpgroup / 6 stages (A/B variant, only
-  // for the text encoder's bias, bias+ReLU and accumulate epilogues with paired CTAs)
+  // accepted for compatibility: the Hopper GEMM has one epilogue schedule
   int epi_groups = 2;
   // Ordered split-K of the accumulate epilogue (x += A.W^T + b with few tiles): zero-initialised device counters, one per
   // (tile, CTA of the pair, epilogue warpgroup); the kernel leaves them zero.  nullptr = never split.  Changes the
@@ -104,7 +111,7 @@ struct ColFilter {
 };
 
 int gemm_topk_chunks(int M, int N, int cta_group, int num_sms);
-// candidate lists per row that gemm_bf16_topk writes for a given n_chunks (two epilogue warpgroups per n-chunk)
+// candidate lists per row that gemm_bf16_topk writes for a given n_chunks (two column halves per n-chunk)
 constexpr int kTopkListsPerChunk = 2;
 inline int gemm_topk_lists(int n_chunks) { return kTopkListsPerChunk * n_chunks; }
 int gemm_bf16_topk(const __nv_bfloat16* A, long long lda, const __nv_bfloat16* W, long long ldw, int M, int N, int K,
@@ -133,13 +140,13 @@ int layernorm_dual(const float* x, const float* gamma, const float* beta, float 
                    long long T, int D, cudaStream_t stream);
 
 // softmax(q k^T / sqrt(64)) v over packed sequences; qkv [T, 3*D] bf16 (q | k | v), out [T, D] bf16
-// impl: 0 = auto (= 2), 1 = mma.sync flash kernel (tests / A-B only), 2 = tcgen05 (any length)
+// impl: 0 = auto (= 2), 1 = mma.sync flash kernel (tests / A-B only), 2 = wgmma (any length)
 int attention_packed(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B, int max_len, int H,
                      long long total_tokens, int impl, int num_sms, __nv_bfloat16* out, cudaStream_t stream);
 int attention_packed_tc(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B, int H, long long total_tokens,
                         __nv_bfloat16* out, int num_sms, cudaStream_t stream);
 
-// Transformer-XL relative-position attention of the Conformer blocks on tcgen05 (attention_relpos_tc.cu):
+// Transformer-XL relative-position attention of the Conformer blocks on wgmma (attention_relpos_tc.cu):
 // score(i,j) = ((q_i+u).k_j + (q_i+v).p[S_center-1-i+j]) / 8; qu / qv = [T, D] bf16 scratch for the biased queries
 int attention_relpos_tc(const __nv_bfloat16* qkv, const __nv_bfloat16* p, const float* u_bias, const float* v_bias,
                         const int32_t* cu_seqlens, int B, int H, long long total_tokens, int Npad, int S_center,

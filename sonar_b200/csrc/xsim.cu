@@ -4,7 +4,7 @@
 //
 // Pipeline for knn(x[n,d], y[m,d], k):
 //   1. l2_normalize: fp32 rows -> unit-norm bf16 rows (+ fp64 norms)                     [HBM-bound]
-//   2. gemm_bf16_topk: tcgen05 GEMM x^ . y^T whose two epilogue warpgroups each keep a running top-16 per row
+//   2. gemm_bf16_topk: wgmma GEMM x^ . y^T whose epilogue keeps, per column half of a tile, a running top-16 per row
 //      in registers (32 candidates per row) -- the n x m similarity matrix is never written  [tensor-bound]
 //   3. exact re-rank of the 16 best of those 32 (by bf16 score) in fp64 from the RAW fp32 embeddings
 //      (cos = <x,y> / (|x||y|)), order (score desc, index asc), keep k                   [gather, L2/HBM]
@@ -147,7 +147,7 @@ static_assert(kXsimCands <= 32, "rerank_kernel maps one candidate to one lane");
 // Few query rows (fewer 256-row tile pairs than SM pairs): the key rows are split into up to 16 chunks swept by different
 // clusters, each writing its own two candidate lists; merge_lists_kernel then keeps the 32 best of them per row.
 static int xsim_chunks(int n, int m) {
-  int c = gemm_topk_chunks(n, m, 2, 148);
+  int c = gemm_topk_chunks(n, m, 2, 0 /* SM count of the device */);
   if (c > 16) {
     const int tiles = (m + 255) / 256, tpc = (tiles + 15) / 16;
     c = (tiles + tpc - 1) / tpc;

@@ -1,4 +1,4 @@
-"""Beam search over the B200 decoder -- the part of fairseq2's ``BeamSearchSeq2SeqGenerator`` [fs2] that
+"""Beam search over the CUDA decoder -- the part of fairseq2's ``BeamSearchSeq2SeqGenerator`` [fs2] that
 ``EmbeddingToTextModelPipeline.predict`` drives (``sonar/inference_pipelines/text.py:315-333``), with the same
 constructor keywords (``beam_size=5, min_gen_len=1, max_gen_len=(1,128), max_seq_len, normalize_scores=True,
 len_penalty=1.0, unk_penalty=0.0``; SURVEY App. C / F8).

@@ -48,7 +48,7 @@ class SpeechToEmbeddingModelPipeline(torch.nn.Module):
             raise FileNotFoundError(f"speech encoder card {encoder!r} cannot be resolved offline; pass a "
                                     "B200SpeechEncoderModel object")
         if fbank_dtype != torch.float32:
-            raise NotImplementedError("the B200 frontend produces fp32 features; the encoder computes in bf16/fp32")
+            raise NotImplementedError("the CUDA frontend produces fp32 features; the encoder computes in bf16/fp32")
         self.device = torch.device(device)
         self.model = encoder.eval()
         self.convert_to_fbank = WaveformToFbank(self.model.device)
@@ -173,7 +173,7 @@ class AudioToFbankDataPipelineBuilder:
         if context.pad_idx != 0:
             raise NotImplementedError("fbank batches are zero padded (the reference default)")
         if context.fbank_dtype != torch.float32:
-            raise NotImplementedError("the B200 frontend produces fp32 features")
+            raise NotImplementedError("the CUDA frontend produces fp32 features")
         frontend = WaveformToFbank(torch.device(context.device))
         root = Path(context.audio_root_dir)
         waves = (_read_wav(root / p) for p in read_tsv_audio_paths(context.data_file, context.audio_path_index))

@@ -2,7 +2,7 @@
 (``/root/reference/sonar/inference_pipelines/text.py:140-269``): same constructor and
 ``predict`` signature, same argument validation, truncation warning, length-sorted
 dynamic bucketing and output-order restoration -- with the model stage running on the
-B200 engine (``sonar_b200.text_encoder.B200TextEncoderModel``).
+CUDA engine (``sonar_b200.text_encoder.B200TextEncoderModel``).
 """
 
 from __future__ import annotations
@@ -34,7 +34,7 @@ _MATMUL_PRECISION = {torch.bfloat16: "medium", torch.float16: "medium", torch.fl
 @contextlib.contextmanager
 def precision_context(dtype: torch.dtype):
     """What the reference wraps every pipeline run in (``text.py:36-54``): torch's float32 matmul precision follows the model
-    dtype for the duration of the call and is put back afterwards.  The sm_100a kernels are not affected by that switch
+    dtype for the duration of the call and is put back afterwards.  The sm_90a kernels are not affected by that switch
     (bf16 operands, fp32 accumulate, always); it is honoured so that torch code a caller runs inside the same ``with`` block
     behaves as it would around the reference."""
     before = torch.get_float32_matmul_precision()
@@ -277,7 +277,7 @@ def _load_decoder_card(name: str, device: Device) -> B200TextDecoderModel:
 
 class EmbeddingToTextModelPipeline(torch.nn.Module):
     """Mirror of ``sonar.inference_pipelines.text.EmbeddingToTextModelPipeline`` (``text.py:272-346``): sentence
-    embeddings -> text with beam search.  ``self.model`` is the B200 decoder itself: the reference wraps it as
+    embeddings -> text with beam search.  ``self.model`` is the CUDA decoder itself: the reference wraps it as
     ``SonarEncoderDecoderModel(DummyEncoderModel, decoder)`` whose ``encode`` only un-squeezes the embedding to
     ``[N,1,D]`` (``sonar/models/sonar_translation/model.py:48-53,81-95``); the generator here does that reshape."""
 
@@ -317,7 +317,7 @@ class EmbeddingToTextModelPipeline(torch.nn.Module):
 
 
 class TextToTextModelPipeline(torch.nn.Module):
-    """Mirror of ``TextToTextModelPipeline`` (``text.py:57-137``): encode with the B200 encoder, decode with the B200
+    """Mirror of ``TextToTextModelPipeline`` (``text.py:57-137``): encode with the CUDA encoder, decode with the CUDA
     decoder.  ``max_seq_len`` is clamped to the decoder's position table like the reference (``:102-107``)."""
 
     def __init__(self, encoder: Union[str, B200TextEncoderModel], decoder: Union[str, B200TextDecoderModel], tokenizer,

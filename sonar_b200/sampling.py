@@ -1,4 +1,4 @@
-"""Sampling generation over the B200 decoder -- the ``sampler=`` branch of ``EmbeddingToTextModelPipeline.predict``
+"""Sampling generation over the CUDA decoder -- the ``sampler=`` branch of ``EmbeddingToTextModelPipeline.predict``
 (``sonar/inference_pipelines/text.py:313-320``): fairseq2's ``SamplingSeq2SeqGenerator`` with a ``TopKSampler`` or
 ``TopPSampler`` [fs2].  fairseq2 is not installable here, so the semantics below are restated from its documented
 behaviour and are **parity unpinned** against it (``oracle/text_decoder.py::sampling_search`` is the CPU restatement the

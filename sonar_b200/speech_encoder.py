@@ -72,9 +72,9 @@ def relative_position_table(max_len: int, dim: int, rows: int) -> Tensor:
 class B200SpeechEncoderModel(torch.nn.Module):
     def __init__(self, config: SonarSpeechEncoderConfig, state_dict: Dict[str, Tensor],
                  device: Union[str, torch.device] = "cuda", *, attn_impl: str = "mma_sync") -> None:
-        """``attn_impl``: relative-position attention kernel -- "mma_sync" (default: the faster one as measured, 488 vs 520 us
-        per layer at 64 x 499 positions plus the 72 us query-bias pre-pass the other needs) or "tcgen05"
-        (``csrc/attention_relpos_tc.cu``: band product, Q K^T and P V on the 5th-gen tensor cores, bitwise independent of the
+        """``attn_impl``: relative-position attention kernel -- "mma_sync" (default; the two have not been timed against each
+        other on the H100) or "tcgen05" (the name the wgmma kernel keeps)
+        (``csrc/attention_relpos_tc.cu``: band product, Q K^T and P V on the tensor cores (wgmma), bitwise independent of the
         batch an utterance is in; ``bench.py`` times both in its speech block)."""
         super().__init__()
         if attn_impl not in ("tcgen05", "mma_sync"):

@@ -80,7 +80,7 @@ class _FrontendInfo:
 
 
 class B200TextDecoderModel(torch.nn.Module):
-    """SONAR text decoder (24 pre-LN layers + final LN + tied projection) on sm_100a kernels."""
+    """SONAR text decoder (24 pre-LN layers + final LN + tied projection) on sm_90a kernels."""
 
     def __init__(self, config: SonarTextDecoderConfig, state_dict: Dict[str, Tensor],
                  device: Union[str, torch.device] = "cuda") -> None:
@@ -89,7 +89,7 @@ class B200TextDecoderModel(torch.nn.Module):
                 or config.no_token_positional_embeddings or not config.normalize_before:
             raise NotImplementedError("sonar_b200 text decoder supports the `basic`/`small` wiring only")
         if config.input_dim not in (None, config.model_dim):
-            raise NotImplementedError("input_dim != model_dim is not supported by the B200 decoder")
+            raise NotImplementedError("input_dim != model_dim is not supported by the CUDA decoder")
         dev = torch.device(device)
         if dev.type != "cuda":
             raise RuntimeError("B200TextDecoderModel needs a CUDA device (there is no CPU path)")

@@ -122,7 +122,7 @@ class _FrontendInfo:
 def _check_supported(cfg: SonarTextEncoderConfig) -> None:
     bad = []
     if cfg.pooling.lower() not in ("mean", "max", "last"):
-        bad.append(f"pooling={cfg.pooling!r} (attention pooling is not on the B200 hot path yet)")
+        bad.append(f"pooling={cfg.pooling!r} (attention pooling is not on the H100 hot path yet)")
     if cfg.activation_fn != "ReLU":
         bad.append(f"activation_fn={cfg.activation_fn!r}")
     if cfg.layernorm_embedding or cfg.no_token_positional_embeddings or cfg.learned_pos:
@@ -136,17 +136,16 @@ def _check_supported(cfg: SonarTextEncoderConfig) -> None:
 
 
 class B200TextEncoderModel(torch.nn.Module):
-    """SONAR text encoder (24-layer pre-LN Transformer + final LN + pooling) on sm_100a kernels."""
+    """SONAR text encoder (24-layer pre-LN Transformer + final LN + pooling) on sm_90a kernels."""
 
     def __init__(self, config: SonarTextEncoderConfig, state_dict: Dict[str, Tensor],
                  device: Union[str, torch.device] = "cuda", *, cta_group: int = 2, ln_fold: Union[bool, int] = False,
                  epi_groups: Optional[int] = None) -> None:
         """``ln_fold=True``: the engine folds every encoder-layer LayerNorm into the GEMMs around it (see
-        ``SbEncoderConfig.ln_fold`` in ``include/sonar_b200.h``); the default runs the separate LayerNorm kernels, which is
-        the faster schedule as measured.  ``epi_groups``: epilogue warpgroups per GEMM CTA -- 1 (six mainloop stages) is the
-        default here: inside the power-capped 24-layer step it is 2 % faster than 2 (five stages), although 2 wins by 9-33 %
-        when a GEMM is timed alone at boost clocks (``bench.py`` A/Bs all of these in every run, ``ab_schedule_variants``).
-        The folded schedules exist with two warpgroups only, so ``None`` means 1 without and 2 with ``ln_fold``."""
+        ``SbEncoderConfig.ln_fold`` in ``include/sonar_b200.h``); the default runs the separate LayerNorm kernels
+        (``bench.py`` A/Bs the schedules in every run, ``ab_schedule_variants``).  ``epi_groups`` is kept for callers that pass
+        it: the Hopper GEMM has one epilogue schedule (its two MMA warpgroups run it), so 1 and 2 select the same kernel;
+        ``None`` means 1 without and 2 with ``ln_fold``."""
         super().__init__()
         if epi_groups is None:
             epi_groups = 2 if int(ln_fold) else 1

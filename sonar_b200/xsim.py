@@ -1,6 +1,6 @@
-"""xsim cosine-margin mining over sentence embeddings on the B200 (BASELINE.json config 5).
+"""xsim cosine-margin mining over sentence embeddings on the H100 (BASELINE.json config 5).
 
-``knn`` / ``knn_bidir`` / ``xsim`` run entirely in ``libsonar_b200.so`` (``sb_xsim_knn``: tcgen05 GEMM with a fused
+``knn`` / ``knn_bidir`` / ``xsim`` run entirely in ``libsonar_b200.so`` (``sb_xsim_knn``: wgmma GEMM with a fused
 running top-k, exact fp64 re-rank; ``sb_xsim_knn_bidir``: both directions from one pass; ``sb_xsim_margin_predict``).
 ``xsim_distributed`` shards the query rows over the ranks of a ``torch.distributed`` group: one all-gather assembles the
 y matrix on every rank (the single exchange step of the path, SURVEY §8e), each rank scores its row block against it once

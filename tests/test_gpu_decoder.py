@@ -37,7 +37,7 @@ def _emb(n, seed=0):
 @pytest.mark.parametrize("n,beam,steps", [(3, 2, 9), (26, 3, 5)])
 def test_teacher_forced_steps_match_oracle(small, cuda_device, n, beam, steps):
     """6 hypothesis rows take the few-rows schedule (skinny GEMMs with the LayerNorms and the cross-attention constant folded
-    in); 78 rows take the tcgen05 tiles with the separate LayerNorm / add kernels."""
+    in); 78 rows take the wgmma tiles with the separate LayerNorm / add kernels."""
     oracle, model = small
     emb = _emb(n)
     g = torch.Generator().manual_seed(1)

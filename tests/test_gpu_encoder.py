@@ -212,7 +212,7 @@ def test_layernorm_folded_into_the_gemms_matches_the_separate_kernels(native_lib
     folded = B200TextEncoderModel(cfg, sd, cuda_device, ln_fold=1)       # both LayerNorms of a layer folded
     folded1 = B200TextEncoderModel(cfg, sd, cuda_device, ln_fold=2)      # only the attention-block LayerNorm
     classic = B200TextEncoderModel(cfg, sd, cuda_device, ln_fold=0)
-    one_group = B200TextEncoderModel(cfg, sd, cuda_device, ln_fold=0, epi_groups=1)  # round-1 epilogue (A/B variant)
+    one_group = B200TextEncoderModel(cfg, sd, cuda_device, ln_fold=0, epi_groups=1)  # option still accepted; selects the same GEMM kernel
     if lens_kind == "dense":
         lens = [128] * 320  # 40 960 rows = 160 pair tiles x 4 n-tiles
     else:

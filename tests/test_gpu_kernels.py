@@ -29,7 +29,7 @@ GEMM_SHAPES = [
     (1000, 1024, 1024),  # out-proj shape, ragged M
     (2048, 3072, 1024),  # QKV shape
     (777, 1024, 8192),   # FFN2 shape (long K), odd M
-    (4096, 8192, 1024),  # FFN1 shape: > 148 tiles -> persistent loop + both TMEM stages
+    (4096, 8192, 1024),  # FFN1 shape: more tiles than SMs -> persistent loop, smem ring wraps
     (1, 256, 64),        # single row
 ]
 
@@ -84,7 +84,7 @@ SKINNY_SHAPES = [(1, 1024, 1024), (7, 3072, 1024), (16, 1024, 8192), (25, 8192, 
 @pytest.mark.parametrize("epilogue", ["bias", "relu", "silu"])
 def test_gemm_skinny_rows(ops, cuda_device, m, n, k, epilogue):
     """M <= 64 goes down the weight-streaming mma.sync path (gemm_skinny.cu): the decoder's small-batch beam step and the
-    speech pooler.  Same contract and tolerances as the tcgen05 path."""
+    speech pooler.  Same contract and tolerances as the wgmma path."""
     a = _rand((m, k), 1.0, 31, cuda_device, torch.bfloat16)
     w = _rand((n, k), 1.0 / math.sqrt(k), 32, cuda_device, torch.bfloat16)
     bias = _rand((n,), 0.5, 33, cuda_device)
@@ -141,7 +141,7 @@ def test_layernorm(ops, cuda_device, t, d):
 
 ATTN_CASES = [([128] * 4, "tcgen05"), ([128] * 4, "mma_sync"), ([1, 2, 17, 64, 65, 128], "tcgen05"),
               ([1, 2, 17, 64, 65, 128], "mma_sync"), ([200, 129, 514], "auto"), ([200, 129, 514], "mma_sync"), ([33], "auto"),
-              ([128] * 700 + [5, 77, 128, 31] * 20, "tcgen05"),  # > 2 x 148 CTAs worth of items: persistent loop
+              ([128] * 700 + [5, 77, 128, 31] * 20, "tcgen05"),  # > 2 x 132 CTAs worth of items: persistent loop
               # multi-tile sentences (online softmax across 128-key tiles) mixed with short ones, uneven item costs per CTA
               ([514, 1, 256, 257, 128, 129, 383, 16, 512, 300] * 4, "tcgen05"),
               ([130] * 40 + [7] * 5, "tcgen05")]
@@ -263,7 +263,7 @@ def test_ln_pool_matches_torch(ops, cuda_device):
 @pytest.mark.parametrize("m,k", [(1000, 1024), (4096, 8192), (300, 256), (77, 1024)])
 def test_gemm_residual_stats(ops, cuda_device, m, k):
     """x += a.W^T + b (fp32, in place) with the bf16 copy and the (mean, M2) partials of the NEW rows: partial 2t + g covers
-    the 128 columns of 256-column tile t that epilogue warpgroup g handles (32-column chunks c with c % 2 == g).
+    column half g (128 columns) of 256-column tile t.
     The rows get a large common offset (mean >> std) so a sum-of-squares style variance would visibly cancel."""
     n = 1024
     a = _rand((m, k), 1.0, 31, cuda_device, torch.bfloat16)
@@ -276,7 +276,7 @@ def test_gemm_residual_stats(ops, cuda_device, m, k):
     ref = x0.double() + a.double() @ w.double().T + bias.double()
     torch.testing.assert_close(x.double(), ref, rtol=1e-5, atol=2e-3)  # fp32 accumulate over K products + fp32 add
     assert torch.equal(h, x.to(torch.bfloat16))                       # the bf16 copy is the rounding of what was stored
-    xc = x.double().view(m, n // 256, 4, 2, 32).transpose(2, 3).reshape(m, n // 128, 128)  # [row, 2t + g, 128]
+    xc = x.double().view(m, n // 128, 128)  # [row, 2t + g, 128]
     torch.testing.assert_close(stats[..., 0].double(), xc.mean(-1), rtol=1e-6, atol=1e-5)
     m2 = ((xc - xc.mean(-1, keepdim=True)) ** 2).sum(-1)
     torch.testing.assert_close(stats[..., 1].double(), m2, rtol=2e-5, atol=1e-4)

@@ -203,10 +203,10 @@ def test_tsv_pipelines_match_the_model_pipelines(speech_small, cuda_device, tmp_
 
 
 def test_relpos_attention_tcgen05_agrees_with_mma_sync_and_is_batch_invariant(native_lib, cuda_device):
-    """The relative-position attention has two implementations: the tcgen05 kernel (attention_relpos_tc.cu: S and the band
-    product on the 5th-gen tensor cores, the Transformer-XL shift as a register barrel shifter, P in tensor memory) and the
-    round-1 mma.sync kernel.  Same model, both kernels, utterances whose position counts sit on and around the 128-row tile
-    edges; both must agree with each other and with the oracle, and the tcgen05 path must give an utterance the same bits
+    """The relative-position attention has two implementations: the wgmma kernel (attention_relpos_tc.cu: S and the band
+    product on the tensor cores (wgmma), the Transformer-XL shift through a skewed shared-memory buffer, P in registers) and the
+    mma.sync kernel.  Same model, both kernels, utterances whose position counts sit on and around the 128-row tile
+    edges; both must agree with each other and with the oracle, and the wgmma path must give an utterance the same bits
     whatever batch it is in (the band window it reads depends on the utterance, not on the batch maximum)."""
     from oracle.speech_encoder import OracleSpeechConfig, OracleSpeechEncoder, make_synthetic_speech_state_dict
     from sonar_b200 import B200SpeechEncoderModel, PaddingMask, SequenceBatch, sonar_speech_encoder_config
@@ -227,10 +227,10 @@ def test_relpos_attention_tcgen05_agrees_with_mma_sync_and_is_batch_invariant(na
     a = tc(batch).sentence_embeddings
     b = ms(batch).sentence_embeddings
     m = parity_metrics(a, b.cpu())
-    print("tcgen05 vs mma.sync rel-pos attention:", m)
+    print("wgmma vs mma.sync rel-pos attention:", m)
     assert m["one_minus_cos_max"] <= 1e-5 and m["rel_l2_max"] <= 5e-3, m
     ref, _, _ = OracleSpeechEncoder(ocfg, sd)(fb, frames)
-    _speech_check(parity_metrics(a, ref), "speech tcgen05 attention vs oracle")
+    _speech_check(parity_metrics(a, ref), "speech wgmma attention vs oracle")
     assert torch.equal(tc(batch).sentence_embeddings, a)  # deterministic
     for i in (1, 4, 7):  # alone in a batch of one: a different batch maximum, the same bits
         n = frames[i]

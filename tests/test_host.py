@@ -86,8 +86,8 @@ def test_library_exports_every_declared_symbol(native_lib):
     assert native_lib.sb_version() >= 100
 
 
-def test_library_contains_blackwell_sass(native_lib):
-    """tcgen05 / TMA must be what the hot GEMM compiles to (B200_PROFILING.md SASS table)."""
+def test_library_contains_hopper_sass(native_lib):
+    """wgmma / TMA must be what the hot GEMM compiles to."""
     import shutil
     import subprocess
 
@@ -97,7 +97,17 @@ def test_library_contains_blackwell_sass(native_lib):
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", str(_lib.lib_path())], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass and "UTMALDG" in sass and "LDTM" in sass
+    assert "HGMMA" in sass and "UTMALDG" in sass and "UTMASTG" in sass
+
+
+def test_wgmma_pipeline_is_not_serialized(native_lib):
+    """ptxas says so in the build log when it has to wait for every wgmma right after issuing it (a function call such as
+    printf in the kernel, a wgmma under a branch, too few registers): the kernels must keep their groups in flight."""
+    from sonar_b200 import build
+
+    log = (build.LIB_DIR / "build.log").read_text()
+    assert "wgmma.mma_async" in log or "gemm_wgmma" in log  # the log is the one of this library
+    assert "wgmma.mma_async instructions are serialized" not in log
 
 
 def test_pipeline_argument_validation():

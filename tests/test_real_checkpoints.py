@@ -7,7 +7,7 @@ checkpoints and the SentencePiece model cannot be downloaded in this environment
                                                 and nllb_langs.txt (one FLORES-200 code per line, NLLB dictionary order)
 
 is set, these tests run the reference's own assertions (/root/reference/tests/integration_tests/test_text_sonar.py) against the
-B200 engine: the cosine-similarity golden of test_text_encoder_sonar_basic (:46-53) and the exact translations of
+CUDA engine: the cosine-similarity golden of test_text_encoder_sonar_basic (:46-53) and the exact translations of
 test_encoder_decoder_translate / test_vec2text_decode (:107-118).  Tolerance for the cosine matrix: the reference asserts
 1e-4 on an fp32 CPU model; the bf16 engine is held to 2e-3 absolute on the cosines (BASELINE.json north_star: embeddings within
 1e-3 cosine of the fp32 path)."""
