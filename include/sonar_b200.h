@@ -184,10 +184,9 @@ int sb_layernorm(const float* x, const float* gamma, const float* beta, float ep
                  void* stream);
 
 /* packed self-attention: qkv bf16 [total_tokens, 3*64*H], cu_seqlens DEVICE int32 [B+1], out bf16 [total_tokens, 64*H].
- * impl 0 = auto (= 2), 1 = mma.sync flash kernel (kept for tests / A-B timing), 2 = wgmma (any length; 128-key
- * tiles with online softmax beyond 128 tokens). */
-int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t max_len, int32_t H,
-                 int64_t total_tokens, int32_t impl, void* out, void* stream);
+ * The wgmma kernel of the encoder: any sequence length (128-key tiles with online softmax beyond 128 tokens). */
+int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t H, int64_t total_tokens, void* out,
+                 void* stream);
 
 /* x[cu[b]+t,:] = embed[ids[b,t],:]*scale + pos[t,:] ; err_flag DEVICE int32 (set to 1 on a bad id) */
 int sb_embed(const int64_t* ids, int64_t ids_row_stride, const int32_t* cu_seqlens, int32_t B, int32_t S,

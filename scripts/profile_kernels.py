@@ -42,7 +42,7 @@ elif which == "attention":
     qkv = torch.randn((T, 3 * D), device=dev, generator=g).to(torch.bfloat16)
     cu = ops.cu_seqlens_of([128] * (T // 128)).to(dev)
     for _ in range(4):
-        ops.attention(qkv, cu, 128, 16)
+        ops.attention(qkv, cu, 16)
 elif which == "layernorm":
     x = torch.randn((T, D), device=dev, generator=g)
     gg, bb = torch.ones(D, device=dev), torch.zeros(D, device=dev)

@@ -104,8 +104,7 @@ _SIGNATURES = {
                                C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "sb_layernorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int64,
                                C.c_int32, C.c_void_p]),
-    "sb_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32,
-                               C.c_void_p, C.c_void_p]),
+    "sb_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     "sb_embed": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,
                            C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_float,

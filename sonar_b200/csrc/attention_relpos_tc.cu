@@ -22,6 +22,7 @@
 // Warpgroup 0 = TMA producer (one thread); Qu | Qv stay for the item, K | Pw and V are single slots that are released as
 // soon as the products reading them have retired, so the next unit's loads run under this unit's softmax.
 
+#include "attention_wgmma.cuh"
 #include "common.cuh"
 #include "sonar_b200_internal.h"
 
@@ -42,12 +43,6 @@ constexpr int kThreads = 384;
 static_assert(kSmemBytes <= 232448, "shared memory budget of one sm_90 block");
 
 enum { Q_FULL = 0, Q_EMPTY, KP_FULL, KP_EMPTY, V_FULL, V_EMPTY, kNumBars };
-
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 
 // The unit sequence of this CTA: items first + i * stride; an item = (query tile, head) of one utterance, expanded
 // into its key tiles.  tile_cu[b] = number of query tiles before utterance b.
@@ -161,7 +156,6 @@ attention_relpos_tc_kernel(const __grid_constant__ CUtensorMap tm_qu, const __gr
     const int cq = 2 * (lane & 3);                 // fragment columns 8 j + cq, + 1
     float* bw = smem_bw + cwg * 64 * kBLd;
     const uint32_t bar_id = 1 + cwg;
-    const float sl2 = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
     const uint32_t sbase = smem_u32(smem);
     float m_run[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_run[2] = {0.f, 0.f};  // l_run: this lane's share of the row sum
     float o[32];
@@ -240,81 +234,14 @@ attention_relpos_tc_kernel(const __grid_constant__ CUtensorMap tm_qu, const __gr
           s[4 * j + 2] += g1[8 * j];
           s[4 * j + 3] += g1[8 * j + 1];
         }
-        // keys >= kv_valid are beyond the utterance: -inf -> probability exactly 0
-        if (kv_valid < 128) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (8 * j + cq >= kv_valid) s[4 * j] = s[4 * j + 2] = -CUDART_INF_F;
-            if (8 * j + cq + 1 >= kv_valid) s[4 * j + 1] = s[4 * j + 3] = -CUDART_INF_F;
-          }
-        }
-        float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
-          mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
-        }
-        float mxs[2];
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-          const float m_new = fmaxf(m_run[r], mx[r]);   // finite: key 0 of every tile is valid
-          alpha[r] = ex2f((m_run[r] - m_new) * sl2);     // 0 on the first key tile (m_run = -inf)
-          m_run[r] = m_new;
-          mxs[r] = m_new * sl2;
-        }
-        float sum[2] = {0.f, 0.f};
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float p0 = ex2f(fmaf(s[4 * j], sl2, -mxs[0])), p1 = ex2f(fmaf(s[4 * j + 1], sl2, -mxs[0]));
-          const float p2 = ex2f(fmaf(s[4 * j + 2], sl2, -mxs[1])), p3 = ex2f(fmaf(s[4 * j + 3], sl2, -mxs[1]));
-          sum[0] += p0 + p1;
-          sum[1] += p2 + p3;
-          pa[j >> 1][(j & 1) * 2] = pack_bf16x2(p0, p1);      // A fragment of k-step j / 2: (row, keys) then (row + 8, keys)
-          pa[j >> 1][(j & 1) * 2 + 1] = pack_bf16x2(p2, p3);
-        }
-        l_run[0] = l_run[0] * alpha[0] + sum[0];
-        l_run[1] = l_run[1] * alpha[1] + sum[1];
+        attn::mask_keys(s, kv_valid, cq);
+        attn::online_softmax(s, m_run, l_run, alpha, pa);
       }
       mbar_wait(&bar[V_FULL], n & 1);
-      if (active) {
-        if (u.kt > 0) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
-            o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
-          }
-        }
-        // all 8 k-steps run (a branch around a wgmma would serialize them): masked keys have P = 0 exactly, and the V rows
-        // behind them are other utterances' finite values or TMA zero fill
-        const uint64_t vd = wgmma_desc_mnmajor_sw128(sbase + kOffV);
-        wgmma_fence_regs(o);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          wgmma_m64n64k16_rs_bt(o, pa[k], vd + uint64_t(k * (2048 >> 4)), (u.kt > 0 || k > 0) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(o);
-      }
+      if (active) attn::pv_accumulate(o, pa, alpha, wgmma_desc_mnmajor_sw128(sbase + kOffV), u.kt == 0);
       __syncwarp();
       if (lane == 0) mbar_arrive(&bar[V_EMPTY]);
-      if (active && last) {
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          float l = l_run[r];
-          l += __shfl_xor_sync(0xffffffffu, l, 1);
-          l += __shfl_xor_sync(0xffffffffu, l, 2);
-          const int qrow = u.q0 + cwg * 64 + fr + 8 * r;
-          if (qrow < u.len) {
-            const float inv = 1.0f / l;
-            uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)(u.tok0 + qrow) * D + u.h * 64 + cq);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) dst[4 * j] = pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
-          }
-        }
-      }
+      if (active && last) attn::store_rows(o, l_run, out, u.tok0, u.q0 + cwg * 64 + fr, u.len, D, u.h * 64 + cq);
       ++n;
       u.advance();
     }

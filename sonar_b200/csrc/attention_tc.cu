@@ -21,9 +21,11 @@
 //   warpgroups 1-2 S, softmax, P.V and the output rows of their 64 queries.  P never touches shared memory: the
 //                  accumulator layout of S is the A-operand register layout of P.V.
 
+#include "attention_wgmma.cuh"
 #include "common.cuh"
 #include "sonar_b200_internal.h"
 
+#include <limits.h>
 #include <math_constants.h>
 
 namespace sb {
@@ -38,12 +40,6 @@ constexpr int kCuSmemInts = 8192;  // cu_seqlens is staged in shared memory when
 constexpr int kSmemBytes = kRingBytes + kBarBytes + kCuSmemInts * 4 + 1024;  // + alignment slack
 static_assert(kSmemBytes <= 232448, "shared memory budget of one sm_90 block");
 constexpr int kThreads = 384;
-
-__device__ __forceinline__ float fast_exp2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 
 // The unit sequence of this CTA: items blockIdx.x + i * gridDim.x, i = 0, 1, ..., each expanded into its
 // (query tile, key tile) units.  Every warp role walks identical copies.
@@ -148,7 +144,6 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, const int32_t* c
     const int cwg = wg_idx - 1;
     const int r_lo = cwg * 64 + (warp & 3) * 16 + (lane >> 2);  // query rows r_lo and r_lo + 8 of the tile
     const int cq = 2 * (lane & 3);                              // fragment columns 8 j + cq, + 1
-    const float sl2 = 0.125f * 1.4426950408889634f;             // 1/sqrt(64) * log2(e)
     float m_run[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_run[2] = {0.f, 0.f};  // l_run: this lane's share of the row sum
     float o[32];
     while (u.valid) {
@@ -175,81 +170,14 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, const int32_t* c
       uint32_t pa[8][4];
       float alpha[2] = {1.f, 1.f};
       if (active) {
-        // keys >= kv_valid are beyond the sentence: -inf -> probability exactly 0
-        if (kv_valid < 128) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (8 * j + cq >= kv_valid) s[4 * j] = s[4 * j + 2] = -CUDART_INF_F;
-            if (8 * j + cq + 1 >= kv_valid) s[4 * j + 1] = s[4 * j + 3] = -CUDART_INF_F;
-          }
-        }
-        float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
-          mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
-        }
-        float mxs[2];
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-          const float m_new = fmaxf(m_run[r], mx[r]);       // finite: key 0 of every tile is valid
-          alpha[r] = fast_exp2((m_run[r] - m_new) * sl2);    // 0 on the first key tile (m_run = -inf)
-          m_run[r] = m_new;
-          mxs[r] = m_new * sl2;
-        }
-        float sum[2] = {0.f, 0.f};
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float p0 = fast_exp2(fmaf(s[4 * j], sl2, -mxs[0])), p1 = fast_exp2(fmaf(s[4 * j + 1], sl2, -mxs[0]));
-          const float p2 = fast_exp2(fmaf(s[4 * j + 2], sl2, -mxs[1])), p3 = fast_exp2(fmaf(s[4 * j + 3], sl2, -mxs[1]));
-          sum[0] += p0 + p1;
-          sum[1] += p2 + p3;
-          pa[j >> 1][(j & 1) * 2] = pack_bf16x2(p0, p1);      // A fragment of k-step j / 2: (row, keys) then (row + 8, keys)
-          pa[j >> 1][(j & 1) * 2 + 1] = pack_bf16x2(p2, p3);
-        }
-        l_run[0] = l_run[0] * alpha[0] + sum[0];
-        l_run[1] = l_run[1] * alpha[1] + sum[1];
+        attn::mask_keys(s, kv_valid, cq);
+        attn::online_softmax(s, m_run, l_run, alpha, pa);
       }
       mbar_wait(&full_v[sv], phv);
-      if (active) {
-        if (u.kt > 0) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
-            o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
-          }
-        }
-        // all 8 k-steps run (a branch around a wgmma would serialize them): masked keys have P = 0 exactly, and the V rows
-        // behind them are other sentences' finite values or TMA zero fill
-        const uint64_t vd = wgmma_desc_mnmajor_sw128(smem_u32(smem_v + sv * kTile));
-        wgmma_fence_regs(o);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          wgmma_m64n64k16_rs_bt(o, pa[k], vd + uint64_t(k * (2048 >> 4)), (u.kt > 0 || k > 0) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(o);
-      }
+      if (active) attn::pv_accumulate(o, pa, alpha, wgmma_desc_mnmajor_sw128(smem_u32(smem_v + sv * kTile)), u.kt == 0);
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_v[sv]);
-      if (active && last) {
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          float l = l_run[r];
-          l += __shfl_xor_sync(0xffffffffu, l, 1);
-          l += __shfl_xor_sync(0xffffffffu, l, 2);
-          const int qrow = u.qt * 128 + r_lo + 8 * r;
-          if (qrow < u.len) {
-            const float inv = 1.0f / l;
-            uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)(u.tok0 + qrow) * D + u.h * 64 + cq);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) dst[4 * j] = pack_bf16x2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
-          }
-        }
-      }
+      if (active && last) attn::store_rows(o, l_run, out, u.tok0, u.qt * 128 + r_lo, u.len, D, u.h * 64 + cq);
       u.advance();
       if (++sq == kQkStages) { sq = 0; phq ^= 1; }
       if (++sv == kVStages) { sv = 0; phv ^= 1; }
@@ -259,9 +187,13 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, const int32_t* c
 
 }  // namespace
 
-int attention_packed_tc(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B, int H, long long total_tokens,
-                        __nv_bfloat16* out, int num_sms, cudaStream_t stream) {
+int attention_packed(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B, int H, long long total_tokens, int num_sms,
+                     __nv_bfloat16* out, cudaStream_t stream) {
   if (B <= 0 || total_tokens <= 0) return 0;
+  if (H <= 0 || (long long)B * H > INT_MAX) {  // the kernel counts (sentence, head) items in an int
+    set_last_error("attention_packed: unsupported B=%d H=%d", B, H);
+    return -1;
+  }
   CUtensorMap tm;
   int rc = make_tmap_2d(&tm, qkv, 2, total_tokens, 3ll * H * 64, 3ll * H * 64, 128, 64);
   if (rc) return rc;

@@ -353,9 +353,25 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_bt(float (&d)[32], const uint
 }
 
 // ----------------------------------------------------------------------------
+// mma.sync (warp-level MMA)
+// ----------------------------------------------------------------------------
+// D[16 x 8] += A[16 x 16] . B[16 x 8] (row.col), bf16 operands in the PTX fragment layouts, fp32 accumulators
+__device__ __forceinline__ void mma_m16n8k16_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
 // ----------------------------------------------------------------------------
 // misc numeric helpers
 // ----------------------------------------------------------------------------
+// 2^x on the SFU (MUFU.EX2), denormals flushed to zero: the softmax numerators of the attention kernels
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);

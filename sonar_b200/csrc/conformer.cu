@@ -85,11 +85,6 @@ __device__ __forceinline__ void ldsm4(uint32_t a, uint32_t& r0, uint32_t& r1, ui
 __device__ __forceinline__ void ldsm4t(uint32_t a, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(a));
 }
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ uint32_t toff(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
 
 // Dynamic shared memory layout of attention_relpos_kernel (bytes).  G (per warp two [16 x 88] fp32 band products, one per
@@ -107,11 +102,6 @@ static_assert(kRpGBytes >= 16384, "Q / output staging lives inside G");
 
 __device__ __forceinline__ void cp4(uint32_t dst, const void* src, bool ok) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(ok ? 4 : 0) : "memory");
-}
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
 }
 
 // score(i,j) = (q_i.k_j + u.k_j + q_i.p[c-1-i+j] + v.p[c-1-i+j]) / 8 with c = S_center.  Per 64-key block the CTA needs the
@@ -258,12 +248,12 @@ attention_relpos_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid
           uint32_t b0, b1, b2, b3;
           ldsm4(sPa + toff(prow, kk * 2 + (mtx & 1)), b0, b1, b2, b3);
           if (use0) {
-            mma16816(ga[a][0][0], qf[0][kk], b0, b1);
-            mma16816(ga[a][0][1], qf[0][kk], b2, b3);
+            mma_m16n8k16_bf16(ga[a][0][0], qf[0][kk], b0, b1);
+            mma_m16n8k16_bf16(ga[a][0][1], qf[0][kk], b2, b3);
           }
           if (use1) {
-            mma16816(ga[a][1][0], qf[1][kk], b0, b1);
-            mma16816(ga[a][1][1], qf[1][kk], b2, b3);
+            mma_m16n8k16_bf16(ga[a][1][0], qf[1][kk], b0, b1);
+            mma_m16n8k16_bf16(ga[a][1][1], qf[1][kk], b2, b3);
           }
         }
       }
@@ -302,8 +292,8 @@ attention_relpos_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid
         ldsm4(sKa + toff(key, kk * 2 + (mtx & 1)), b0, b1, b2, b3);
 #pragma unroll
         for (int m = 0; m < 2; ++m) {
-          mma16816(s[m][jp * 2], qf[m][kk], b0, b1);
-          mma16816(s[m][jp * 2 + 1], qf[m][kk], b2, b3);
+          mma_m16n8k16_bf16(s[m][jp * 2], qf[m][kk], b0, b1);
+          mma_m16n8k16_bf16(s[m][jp * 2 + 1], qf[m][kk], b2, b3);
         }
       }
     }
@@ -372,8 +362,8 @@ attention_relpos_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid
         ldsm4t(sVa + toff(key, jp * 2 + (mtx >> 1)), b0, b1, b2, b3);
 #pragma unroll
         for (int m = 0; m < 2; ++m) {
-          mma16816(o[m][jp * 2], pf[m][kk], b0, b1);
-          mma16816(o[m][jp * 2 + 1], pf[m][kk], b2, b3);
+          mma_m16n8k16_bf16(o[m][jp * 2], pf[m][kk], b0, b1);
+          mma_m16n8k16_bf16(o[m][jp * 2 + 1], pf[m][kk], b2, b3);
         }
       }
     }

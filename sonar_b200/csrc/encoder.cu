@@ -115,7 +115,7 @@ static Workspace carve(const SbEncoder* e, int32_t max_batch, int64_t max_tokens
 extern "C" {
 
 const char* sb_last_error(void) { return g_err; }
-int sb_version(void) { return 102; }
+int sb_version(void) { return 103; }
 
 int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbEncoder** out) {
   if (!cfg || !w || !out) { set_last_error("sb_encoder_create: null argument"); return SB_ERR_INVALID; }
@@ -278,13 +278,11 @@ int sb_encoder_forward(SbEncoder* e, const int64_t* ids, int64_t ids_row_stride,
   SB_CUDA_CHECK(cudaEventSynchronize(e->ev[slot]));  // only blocks if 8 forwards are still in flight
   int32_t* cu_h = e->pinned + (size_t)slot * SbEncoder::kSlotInts;
   long long T = 0;
-  int max_len = 0;
   cu_h[0] = 0;
   for (int b = 0; b < B; ++b) {
     const int len = seq_lens_host ? seq_lens_host[b] : S;
     if (len < 0 || len > S) { set_last_error("sb_encoder_forward: seq_lens[%d]=%d outside [0,%d]", b, len, S); return SB_ERR_INVALID; }
     T += len;
-    if (len > max_len) max_len = len;
     if (T > 0x7fffffffll) { set_last_error("sb_encoder_forward: too many tokens"); return SB_ERR_INVALID; }
     cu_h[b + 1] = (int32_t)T;
   }
@@ -337,7 +335,7 @@ int sb_encoder_forward(SbEncoder* e, const int64_t* ids, int64_t ids_row_stride,
     rc = gemm_bf16(g, stream);
     g.lf = LnFold();
     if (rc) return rc;
-    if ((rc = attention_packed(w.qkv, w.cu, B, max_len, H, T, 0, e->num_sms, w.h, stream))) return rc;
+    if ((rc = attention_packed(w.qkv, w.cu, B, H, T, e->num_sms, w.h, stream))) return rc;
     g.A = w.h; g.lda = D; g.W = reinterpret_cast<const __nv_bfloat16*>(L.wo); g.ldw = D;
     g.C = w.x; g.ldc = D; g.out_fp32 = 1; g.bias = L.bo; g.residual = w.x; g.ldr = D;
     g.N = D; g.K = D; g.epi = EPI_BIAS_RESIDUAL;
@@ -513,14 +511,14 @@ int sb_layernorm(const float* x, const float* gamma, const float* beta, float ep
                         reinterpret_cast<cudaStream_t>(stream));
 }
 
-int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t max_len, int32_t H,
-                 int64_t total_tokens, int32_t impl, void* out, void* stream) {
+int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t H, int64_t total_tokens, void* out,
+                 void* stream) {
   if (!qkv || !cu_seqlens || !out) { set_last_error("sb_attention: null pointer"); return SB_ERR_INVALID; }
   int dev = 0, sms = 0;
   SB_CUDA_CHECK(cudaGetDevice(&dev));
   SB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  return attention_packed(reinterpret_cast<const __nv_bfloat16*>(qkv), cu_seqlens, B, max_len, H, total_tokens, impl,
-                          sms, reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<cudaStream_t>(stream));
+  return attention_packed(reinterpret_cast<const __nv_bfloat16*>(qkv), cu_seqlens, B, H, total_tokens, sms,
+                          reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<cudaStream_t>(stream));
 }
 
 int sb_embed(const int64_t* ids, int64_t ids_row_stride, const int32_t* cu_seqlens, int32_t B, int32_t S,

@@ -35,13 +35,6 @@ __device__ __forceinline__ void st_shared_cluster_f32(const float* local_addr, u
       : "memory");
 }
 
-__device__ __forceinline__ void mma16816_f32(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                             uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
 // MT = number of 16-row activation tiles (M <= 16 * MT); UNROLL = 32-element chunks in flight per lane;
 // gridDim.y = cluster size = number of K splits (1..8)
 template <int MT, int UNROLL, typename OutT>
@@ -91,8 +84,10 @@ gemm_skinny_kernel(const __nv_bfloat16* __restrict__ A, long long lda, const __n
     for (int u = 0; u < kUnroll; ++u)
 #pragma unroll
       for (int i = 0; i < MT; ++i) {
-        mma16816_f32(acc[i], a4[u][i][0].x, a4[u][i][1].x, a4[u][i][0].y, a4[u][i][1].y, w4[u].x, w4[u].y);
-        mma16816_f32(acc[i], a4[u][i][0].z, a4[u][i][1].z, a4[u][i][0].w, a4[u][i][1].w, w4[u].z, w4[u].w);
+        const uint32_t lo[4] = {a4[u][i][0].x, a4[u][i][1].x, a4[u][i][0].y, a4[u][i][1].y};
+        const uint32_t hi[4] = {a4[u][i][0].z, a4[u][i][1].z, a4[u][i][0].w, a4[u][i][1].w};
+        mma_m16n8k16_bf16(acc[i], lo, w4[u].x, w4[u].y);
+        mma_m16n8k16_bf16(acc[i], hi, w4[u].z, w4[u].w);
       }
   }
   // accumulator fragment: c0,c1 -> (row g, cols 2t,2t+1); c2,c3 -> (row g+8, cols 2t,2t+1)

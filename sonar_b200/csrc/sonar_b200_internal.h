@@ -139,12 +139,10 @@ int layernorm_bf16(const float* x, const float* gamma, const float* beta, float 
 int layernorm_dual(const float* x, const float* gamma, const float* beta, float eps, float* y32, __nv_bfloat16* y16,
                    long long T, int D, cudaStream_t stream);
 
-// softmax(q k^T / sqrt(64)) v over packed sequences; qkv [T, 3*D] bf16 (q | k | v), out [T, D] bf16
-// impl: 0 = auto (= 2), 1 = mma.sync flash kernel (tests / A-B only), 2 = wgmma (any length)
-int attention_packed(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B, int max_len, int H,
-                     long long total_tokens, int impl, int num_sms, __nv_bfloat16* out, cudaStream_t stream);
-int attention_packed_tc(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B, int H, long long total_tokens,
-                        __nv_bfloat16* out, int num_sms, cudaStream_t stream);
+// softmax(q k^T / sqrt(64)) v over packed sequences of any length on wgmma (attention_tc.cu); qkv [T, 3*D] bf16
+// (q | k | v), out [T, D] bf16
+int attention_packed(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B, int H, long long total_tokens, int num_sms,
+                     __nv_bfloat16* out, cudaStream_t stream);
 
 // Transformer-XL relative-position attention of the Conformer blocks on wgmma (attention_relpos_tc.cu):
 // score(i,j) = ((q_i+u).k_j + (q_i+v).p[S_center-1-i+j]) / 8; qu / qv = [T, D] bf16 scratch for the biased queries

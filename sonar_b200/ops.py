@@ -72,9 +72,6 @@ def cu_seqlens_of(seq_lens) -> Tensor:
     return cu
 
 
-ATTENTION_IMPLS = {"auto": 0, "mma_sync": 1, "tcgen05": 2}
-
-
 def fold_layernorm(w: Tensor, bias: Tensor, gamma: Tensor, beta: Tensor):
     """LayerNorm folding, weight side: -> (Wf bf16 [N,K], colsum fp32 [N], bias_f fp32 [N])."""
     _need_cuda(w, bias, gamma, beta)
@@ -132,7 +129,7 @@ def gemm_ln_consumer(a: Tensor, wf: Tensor, bias_f: Tensor, colsum: Tensor, stat
     return out
 
 
-def attention(qkv: Tensor, cu_seqlens: Tensor, max_len: int, num_heads: int, impl: str = "auto") -> Tensor:
+def attention(qkv: Tensor, cu_seqlens: Tensor, num_heads: int) -> Tensor:
     """Packed bidirectional MHA: qkv bf16 [T, 3*64*H] -> bf16 [T, 64*H]."""
     _need_cuda(qkv, cu_seqlens)
     assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and cu_seqlens.dtype == torch.int32
@@ -140,8 +137,8 @@ def attention(qkv: Tensor, cu_seqlens: Tensor, max_len: int, num_heads: int, imp
     d = 64 * num_heads
     assert qkv.shape[1] == 3 * d
     out = torch.empty((t, d), dtype=torch.bfloat16, device=qkv.device)
-    rc = _lib.load().sb_attention(qkv.data_ptr(), cu_seqlens.data_ptr(), cu_seqlens.numel() - 1, max_len,
-                                  num_heads, t, ATTENTION_IMPLS[impl], out.data_ptr(), _stream())
+    rc = _lib.load().sb_attention(qkv.data_ptr(), cu_seqlens.data_ptr(), cu_seqlens.numel() - 1, num_heads, t,
+                                  out.data_ptr(), _stream())
     _lib.check(rc, "sb_attention")
     return out
 
