@@ -76,8 +76,6 @@ typedef struct SbEncoderConfig {
                           * 2 = fold only the attention-block LayerNorm (FFN2 emits, QKV applies); the FFN-block LayerNorm
                           *     stays a kernel (the out-projection is HBM-bound, its epilogue has no slack for the extra work);
                           * 0 = separate LayerNorm kernels */
-  int32_t epi_groups;    /* 0, 1 or 2; accepted for compatibility (1 needs ln_fold = 0 and CTA pairs): the Hopper GEMM
-                          *     has one epilogue schedule */
 } SbEncoderConfig;
 
 /* All pointers are DEVICE pointers and stay owned by the caller (must outlive the handle).

@@ -23,7 +23,7 @@ class SbEncoderConfig(C.Structure):
         ("model_dim", C.c_int32), ("num_layers", C.c_int32), ("num_heads", C.c_int32),
         ("ffn_inner_dim", C.c_int32), ("vocab_size", C.c_int64), ("pos_rows", C.c_int32),
         ("pooling", C.c_int32), ("ln_eps", C.c_float), ("embed_scale", C.c_float),
-        ("cta_group", C.c_int32), ("num_sms", C.c_int32), ("ln_fold", C.c_int32), ("epi_groups", C.c_int32),
+        ("cta_group", C.c_int32), ("num_sms", C.c_int32), ("ln_fold", C.c_int32),
     ]
 
 

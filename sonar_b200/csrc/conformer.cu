@@ -25,8 +25,6 @@
 namespace sb {
 namespace {
 
-inline size_t align_up_c(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 constexpr int kFeat = 160, kFeatPad = 192;
 
 // ---------------------------------------------------------------------------------------------
@@ -591,25 +589,23 @@ SpWs carve_sp(const SbSpeechEncoder* e, int B, long long T, int smax, void* base
   const size_t D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, Fp = e->cfg.pooler_ffn_inner_dim, H = e->cfg.num_heads;
   const size_t np = npad_of(smax);
   size_t wide = F > 3 * D ? F : 3 * D;
-  uint8_t* p = reinterpret_cast<uint8_t*>(base);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { uint8_t* q = p + off; off = align_up_c(off + bytes, 1024); return q; };
+  Carver c(base);
   SpWs w;
   const size_t t = (size_t)T;
-  w.a192 = reinterpret_cast<__nv_bfloat16*>(take(t * kFeatPad * 2));
-  w.x = reinterpret_cast<float*>(take(t * D * 4));
-  w.h = reinterpret_cast<__nv_bfloat16*>(take(t * D * 2));
-  w.big = reinterpret_cast<__nv_bfloat16*>(take(t * wide * 2));
-  w.p = reinterpret_cast<__nv_bfloat16*>(take(np * D * 2));
-  w.vp = reinterpret_cast<float*>(take(H * np * 4));
-  w.qu = reinterpret_cast<__nv_bfloat16*>(take(t * D * 2));  // bf16(q + u), bf16(q + v): A operands of the wgmma attention
-  w.qv = reinterpret_cast<__nv_bfloat16*>(take(t * D * 2));
-  w.e = reinterpret_cast<__nv_bfloat16*>(take(t * D * 2));
-  w.px = reinterpret_cast<float*>(take((size_t)B * D * 4));
-  w.ph = reinterpret_cast<__nv_bfloat16*>(take((size_t)B * D * 2));
-  w.pt = reinterpret_cast<__nv_bfloat16*>(take((size_t)B * (Fp > D ? Fp : D) * 2));
-  w.pq = reinterpret_cast<__nv_bfloat16*>(take((size_t)B * D * 2));
-  w.bytes = off;
+  w.a192 = c.take<__nv_bfloat16>(t * kFeatPad * 2);
+  w.x = c.take<float>(t * D * 4);
+  w.h = c.take<__nv_bfloat16>(t * D * 2);
+  w.big = c.take<__nv_bfloat16>(t * wide * 2);
+  w.p = c.take<__nv_bfloat16>(np * D * 2);
+  w.vp = c.take<float>(H * np * 4);
+  w.qu = c.take<__nv_bfloat16>(t * D * 2);  // bf16(q + u), bf16(q + v): A operands of the wgmma attention
+  w.qv = c.take<__nv_bfloat16>(t * D * 2);
+  w.e = c.take<__nv_bfloat16>(t * D * 2);
+  w.px = c.take<float>((size_t)B * D * 4);
+  w.ph = c.take<__nv_bfloat16>((size_t)B * D * 2);
+  w.pt = c.take<__nv_bfloat16>((size_t)B * (Fp > D ? Fp : D) * 2);
+  w.pq = c.take<__nv_bfloat16>((size_t)B * D * 2);
+  w.bytes = c.off;
   return w;
 }
 
@@ -632,32 +628,25 @@ int sb_speech_encoder_create(const SbSpeechConfig* cfg, const SbSpeechWeights* w
     set_last_error("sb_speech_encoder_create: missing weight pointer");
     return SB_ERR_INVALID;
   }
-  int dev = 0, n_gpu = 0;
-  if (cudaGetDeviceCount(&n_gpu) != cudaSuccess || n_gpu == 0) {
-    set_last_error("sb_speech_encoder_create: no CUDA device (this engine has no CPU path)");
-    return SB_ERR_CUDA;
-  }
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  SB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 9) { set_last_error("sb_speech_encoder_create: needs a Hopper H100-class GPU (sm_90)"); return SB_ERR_CUDA; }
+  for (int i = 0; i < cfg->num_layers; ++i)
+    if (has_null_pointer(w->layers[i])) {
+      set_last_error("sb_speech_encoder_create: conformer layer %d has a null weight pointer", i);
+      return SB_ERR_INVALID;
+    }
+  for (int i = 0; i < cfg->pooler_layers; ++i)
+    if (has_null_pointer(w->pooler[i])) {
+      set_last_error("sb_speech_encoder_create: pooler layer %d has a null weight pointer", i);
+      return SB_ERR_INVALID;
+    }
+  int num_sms = 0;
+  if (int rc = require_hopper("sb_speech_encoder_create", &num_sms)) return rc;
   SbSpeechEncoder* e = new (std::nothrow) SbSpeechEncoder();
   if (!e) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   e->cfg = *cfg;
   e->w = *w;
   e->layers.assign(w->layers, w->layers + cfg->num_layers);
   e->pool.assign(w->pooler, w->pooler + cfg->pooler_layers);
-  for (auto& l : e->layers) {
-    const void* const* ptrs = reinterpret_cast<const void* const*>(&l);
-    for (size_t i = 0; i < sizeof(l) / sizeof(void*); ++i)
-      if (!ptrs[i]) { set_last_error("sb_speech_encoder_create: null conformer weight"); delete e; return SB_ERR_INVALID; }
-  }
-  for (auto& l : e->pool) {
-    const void* const* ptrs = reinterpret_cast<const void* const*>(&l);
-    for (size_t i = 0; i < sizeof(l) / sizeof(void*); ++i)
-      if (!ptrs[i]) { set_last_error("sb_speech_encoder_create: null pooler weight"); delete e; return SB_ERR_INVALID; }
-  }
-  e->num_sms = prop.multiProcessorCount;
+  e->num_sms = num_sms;
   *out = e;
   return SB_OK;
 }
@@ -670,7 +659,7 @@ int sb_speech_encoder_workspace_bytes(const SbSpeechEncoder* e, int32_t B, int64
     set_last_error("sb_speech_encoder_workspace_bytes: bad argument");
     return SB_ERR_INVALID;
   }
-  *bytes = carve_sp(e, B, total_positions, max_positions, nullptr).bytes + 1024;
+  *bytes = carve_sp(e, B, total_positions, max_positions, nullptr).bytes + kWorkspaceAlign;
   return SB_OK;
 }
 
@@ -697,12 +686,10 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
                    smax, relpos_rows);
     return SB_ERR_INVALID;
   }
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023);
-  SpWs w = carve_sp(e, B, T, smax, reinterpret_cast<void*>(base));
-  if (base - reinterpret_cast<uintptr_t>(workspace) + w.bytes > workspace_bytes) {
-    set_last_error("sb_speech_encoder_forward: workspace too small");
-    return SB_ERR_INVALID;
-  }
+  SpWs w;
+  int rc = bind_workspace("sb_speech_encoder_forward", workspace, workspace_bytes, &w,
+                          [&](void* p) { return carve_sp(e, B, T, smax, p); });
+  if (rc) return rc;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   const int D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, H = e->cfg.num_heads, Fp = e->cfg.pooler_ffn_inner_dim;
   const float eps = e->cfg.ln_eps;
@@ -710,20 +697,15 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
   if (first_use_on_device(attr_set)) {
     SB_CUDA_CHECK(cudaFuncSetAttribute(attention_relpos_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRpSmem));
   }
-  int rc;
   // TMA views for the rel-pos attention: 64 x 64 boxes of the packed qkv rows [T, 3D] and of the projected table [Npad, D]
   CUtensorMap tm_qkv, tm_p;
   if ((rc = make_tmap_2d(&tm_qkv, w.big, 2, T, 3ll * D, 3ll * D, 64, 64))) return rc;
   if ((rc = make_tmap_2d(&tm_p, w.p, 2, Npad, D, D, 64, 64))) return rc;
-  GemmArgs g;
-  g.allow_skinny = 1;
-  g.cta_group = 2;
-  g.num_sms = e->num_sms;
-  auto gemm = [&](const __nv_bfloat16* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int fp32,
-                  const float* bias, int M, int N, int K, int epi) -> int {
-    g.A = A; g.lda = lda; g.W = reinterpret_cast<const __nv_bfloat16*>(W); g.ldw = ldw; g.C = C; g.ldc = ldc;
-    g.out_fp32 = fp32; g.bias = bias; g.residual = (epi == EPI_BIAS_RESIDUAL) ? C : nullptr; g.ldr = ldc;
-    g.M = M; g.N = N; g.K = K; g.epi = epi;
+  // every GEMM may take the weight-streaming path (the pooler's B rows)
+  auto gemm = [&](const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int fp32,
+                  const float* bias, int M, int N, int K, int epi) {
+    GemmArgs g = gemm_args(A, lda, W, ldw, C, ldc, fp32, bias, M, N, K, epi, e->num_sms);
+    g.allow_skinny = 1;
     return gemm_bf16(g, stream);
   };
   // ---- frontend ----
@@ -741,7 +723,7 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
     // (b) relative-position self-attention
     if ((rc = layernorm_bf16(w.x, L.attn_ln_g, L.attn_ln_b, eps, w.h, T, D, stream))) return rc;
     if ((rc = gemm(w.h, D, L.wqkv, D, w.big, 3 * D, 0, L.bqkv, (int)T, 3 * D, D, EPI_BIAS))) return rc;
-    if ((rc = gemm(reinterpret_cast<const __nv_bfloat16*>(relpos_table), D, L.wr, D, w.p, D, 0, e->w.zeros, Npad, D, D, EPI_BIAS))) return rc;
+    if ((rc = gemm(relpos_table, D, L.wr, D, w.p, D, 0, e->w.zeros, Npad, D, D, EPI_BIAS))) return rc;
     if (e->cfg.attn_impl == 1 || B > 2047) {  // mma.sync kernel (A/B runs, second implementation in the tests)
       relpos_bias_kernel<<<dim3((unsigned)((Npad + 7) / 8), (unsigned)H), 256, 0, stream>>>(w.p, L.v_bias, Npad, H, w.vp);
       SB_CUDA_CHECK(cudaGetLastError());

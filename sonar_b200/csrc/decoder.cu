@@ -29,8 +29,6 @@
 
 namespace sb {
 
-static inline size_t align_up_d(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 // x[r,:] = E[token[r],:] * scale + pos[t,:]      (one warp per row)
 __global__ void __launch_bounds__(256)
 decode_embed_kernel(const int64_t* __restrict__ tokens, const __nv_bfloat16* __restrict__ embed, long long vocab,
@@ -63,24 +61,8 @@ decode_embed_kernel(const int64_t* __restrict__ tokens, const __nv_bfloat16* __r
   }
 }
 
-// x[r,:] += c[r / beam, :]   (fp32, one warp per row)
-__global__ void __launch_bounds__(256)
-add_sentence_const_kernel(float* __restrict__ x, const float* __restrict__ c, int R, int beam, int D) {
-  const int r = blockIdx.x * 8 + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (r >= R) return;
-  float4* xr = reinterpret_cast<float4*>(x + (long long)r * D);
-  const float4* cr = reinterpret_cast<const float4*>(c + (long long)(r / beam) * D);
-  for (int q = lane; q < D / 4; q += 32) {
-    float4 a = xr[q];
-    const float4 b = __ldg(cr + q);
-    a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
-    xr[q] = a;
-  }
-}
-
 // x[r,:] += c[r / beam, :], then h[r,:] = LayerNorm(x[r,:]) in bf16: the collapsed cross-attention residual and the FFN
-// LayerNorm in one pass over the row (bit-identical to add_sentence_const_kernel followed by layernorm_bf16).
+// LayerNorm in one pass over the row (D = 128 * nvec, nvec <= kMaxVec).
 __global__ void __launch_bounds__(256)
 add_const_layernorm_kernel(float* __restrict__ x, const float* __restrict__ c, int R, int beam, int D,
                            const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
@@ -334,7 +316,7 @@ namespace {
 constexpr long long kSplitkFlags = 4096;  // >= 4 * (tile pairs of an [R, D] residual GEMM) whenever splitting can pay
 
 struct DecWs {
-  int32_t* err_flag;
+  int32_t* err_flag;      // first buffer: sb_decoder_check_inputs finds it at the workspace base
   int* splitk_flags;      // [kSplitkFlags] hand-over counters of the split-K residual GEMMs (zeroed by sb_decoder_begin)
   float* x;               // [R, D] fp32 residual stream of the current step
   __nv_bfloat16* h;       // [R, D]
@@ -355,44 +337,38 @@ struct DecWs {
 DecWs carve_dec(const SbDecoder* d, int N, int beam, int Tmax, void* base) {
   const size_t D = d->cfg.model_dim, F = d->cfg.ffn_inner_dim, L = d->cfg.num_layers;
   const size_t R = (size_t)N * beam;
-  uint8_t* p = reinterpret_cast<uint8_t*>(base);
-  size_t off = 0;
+  Carver c(base);
   DecWs w;
-  auto take = [&](size_t bytes) { uint8_t* q = p + off; off = align_up_d(off + bytes, 1024); return q; };
   w.n_chunks = gemm_topk_chunks((int)R, (int)d->cfg.vocab_size, 2, d->num_sms);
-  w.err_flag = reinterpret_cast<int32_t*>(take(256));
-  w.splitk_flags = reinterpret_cast<int*>(take(kSplitkFlags * sizeof(int)));
-  w.x = reinterpret_cast<float*>(take(R * D * 4));
-  w.h = reinterpret_cast<__nv_bfloat16*>(take(R * D * 2));
-  w.qkv = reinterpret_cast<__nv_bfloat16*>(take(R * 3 * D * 2));
-  w.f = reinterpret_cast<__nv_bfloat16*>(take(R * F * 2));
-  w.cross = reinterpret_cast<float*>(take(L * (size_t)N * D * 4));
-  w.ebf = reinterpret_cast<__nv_bfloat16*>(take((size_t)N * D * 2));
-  w.vtmp = reinterpret_cast<__nv_bfloat16*>(take((size_t)N * D * 2));
+  w.err_flag = c.take<int32_t>(256);
+  w.splitk_flags = c.take<int>(kSplitkFlags * sizeof(int));
+  w.x = c.take<float>(R * D * 4);
+  w.h = c.take<__nv_bfloat16>(R * D * 2);
+  w.qkv = c.take<__nv_bfloat16>(R * 3 * D * 2);
+  w.f = c.take<__nv_bfloat16>(R * F * 2);
+  w.cross = c.take<float>(L * (size_t)N * D * 4);
+  w.ebf = c.take<__nv_bfloat16>((size_t)N * D * 2);
+  w.vtmp = c.take<__nv_bfloat16>((size_t)N * D * 2);
   const size_t n_lists = (size_t)gemm_topk_lists(w.n_chunks);
-  w.cand_val = reinterpret_cast<float*>(take(R * n_lists * kTopkCandidates * 4));
-  w.cand_idx = reinterpret_cast<int*>(take(R * n_lists * kTopkCandidates * 4));
-  w.lse_part = reinterpret_cast<float*>(take(R * n_lists * 2 * 4));
-  w.kcache = reinterpret_cast<__nv_bfloat16*>(take(L * R * (size_t)Tmax * D * 2));
-  w.vcache = reinterpret_cast<__nv_bfloat16*>(take(L * R * (size_t)Tmax * D * 2));
-  w.bytes = off;
+  w.cand_val = c.take<float>(R * n_lists * kTopkCandidates * 4);
+  w.cand_idx = c.take<int>(R * n_lists * kTopkCandidates * 4);
+  w.lse_part = c.take<float>(R * n_lists * 2 * 4);
+  w.kcache = c.take<__nv_bfloat16>(L * R * (size_t)Tmax * D * 2);
+  w.vcache = c.take<__nv_bfloat16>(L * R * (size_t)Tmax * D * 2);
+  w.bytes = c.off;
   return w;
 }
 
-int check_ws(const SbDecoder* d, int N, int beam, int Tmax, void* workspace, size_t workspace_bytes, DecWs* out) {
-  if (!d || !workspace) { set_last_error("sb_decoder: null argument"); return SB_ERR_INVALID; }
+int check_ws(const char* who, const SbDecoder* d, int N, int beam, int Tmax, void* workspace, size_t workspace_bytes,
+             DecWs* out) {
+  if (!d || !workspace) { set_last_error("%s: null argument", who); return SB_ERR_INVALID; }
   if (N <= 0 || beam <= 0 || Tmax <= 0 || Tmax > d->cfg.pos_rows) {
-    set_last_error("sb_decoder: bad N=%d beam=%d max_len=%d (position table has %d rows)", N, beam, Tmax, d->cfg.pos_rows);
+    set_last_error("%s: bad N=%d beam=%d max_len=%d (position table has %d rows)", who, N, beam, Tmax, d->cfg.pos_rows);
     return SB_ERR_INVALID;
   }
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023);
-  *out = carve_dec(d, N, beam, Tmax, reinterpret_cast<void*>(base));
-  if (base - reinterpret_cast<uintptr_t>(workspace) + out->bytes > workspace_bytes) {
-    set_last_error("sb_decoder: workspace too small (%zu given, %zu needed)", workspace_bytes,
-                   (size_t)(base - reinterpret_cast<uintptr_t>(workspace)) + out->bytes);
-    return SB_ERR_INVALID;
-  }
-  if (gemm_topk_lists(out->n_chunks) > 256) { set_last_error("sb_decoder: vocabulary split into too many chunks"); return SB_ERR_INVALID; }
+  auto carve = [&](void* p) { return carve_dec(d, N, beam, Tmax, p); };
+  if (int rc = bind_workspace(who, workspace, workspace_bytes, out, carve)) return rc;
+  if (gemm_topk_lists(out->n_chunks) > 256) { set_last_error("%s: vocabulary split into too many chunks", who); return SB_ERR_INVALID; }
   return SB_OK;
 }
 
@@ -408,6 +384,7 @@ int sb_decoder_create(const SbDecoderConfig* cfg, const SbDecoderWeights* w, SbD
     set_last_error("sb_decoder_create: need model_dim %% 256 == 0 (<= 1024), head_dim 64, ffn %% 256 == 0");
     return SB_ERR_INVALID;
   }
+  static_assert(128 * kMaxVec >= 1024, "add_const_layernorm_kernel holds a row of up to 1024 columns in registers");
   if (cfg->input_dim != D) {
     set_last_error("sb_decoder_create: input_dim (%d) must equal model_dim (%d)", cfg->input_dim, D);
     return SB_ERR_INVALID;
@@ -421,18 +398,13 @@ int sb_decoder_create(const SbDecoderConfig* cfg, const SbDecoderWeights* w, SbD
     set_last_error("sb_decoder_create: missing weight pointer");
     return SB_ERR_INVALID;
   }
-  int dev = 0, n_gpu = 0;
-  if (cudaGetDeviceCount(&n_gpu) != cudaSuccess || n_gpu == 0) {
-    set_last_error("sb_decoder_create: no CUDA device (this engine has no CPU path)");
-    return SB_ERR_CUDA;
-  }
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  SB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 9) {
-    set_last_error("sb_decoder_create: sm_90a kernels need a Hopper H100-class GPU (found sm_%d%d)", prop.major, prop.minor);
-    return SB_ERR_CUDA;
-  }
+  for (int i = 0; i < cfg->num_layers; ++i)
+    if (has_null_pointer(w->layers[i])) {
+      set_last_error("sb_decoder_create: layer %d has a null weight pointer", i);
+      return SB_ERR_INVALID;
+    }
+  int num_sms = 0;
+  if (int rc = require_hopper("sb_decoder_create", &num_sms)) return rc;
   SbDecoder* d = new (std::nothrow) SbDecoder();
   if (!d) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   d->cfg = *cfg;
@@ -441,18 +413,7 @@ int sb_decoder_create(const SbDecoderConfig* cfg, const SbDecoderWeights* w, SbD
   d->final_ln_g = w->final_ln_g;
   d->final_ln_b = w->final_ln_b;
   d->layers.assign(w->layers, w->layers + cfg->num_layers);
-  for (int i = 0; i < cfg->num_layers; ++i) {
-    const SbDecoderLayerWeights& l = d->layers[i];
-    const void* ptrs[] = {l.wqkv, l.bqkv, l.wo, l.bo, l.cross_wv, l.cross_bv, l.cross_wo, l.cross_bo, l.w1, l.b1,
-                          l.w2, l.b2, l.ln1_g, l.ln1_b, l.ln3_g, l.ln3_b};
-    for (const void* q : ptrs)
-      if (!q) {
-        set_last_error("sb_decoder_create: layer %d has a null weight pointer", i);
-        delete d;
-        return SB_ERR_INVALID;
-      }
-  }
-  d->num_sms = prop.multiProcessorCount;
+  d->num_sms = num_sms;
   *out = d;
   return SB_OK;
 }
@@ -464,14 +425,14 @@ int sb_decoder_workspace_bytes(const SbDecoder* d, int32_t num_sentences, int32_
     set_last_error("sb_decoder_workspace_bytes: bad argument");
     return SB_ERR_INVALID;
   }
-  *bytes = carve_dec(d, num_sentences, beam, max_len, nullptr).bytes + 1024;
+  *bytes = carve_dec(d, num_sentences, beam, max_len, nullptr).bytes + kWorkspaceAlign;
   return SB_OK;
 }
 
 int sb_decoder_begin(SbDecoder* d, const float* embeddings, int32_t N, int32_t beam, int32_t max_len, void* workspace,
                      size_t workspace_bytes, void* stream_v) {
   DecWs w;
-  int rc = check_ws(d, N, beam, max_len, workspace, workspace_bytes, &w);
+  int rc = check_ws("sb_decoder_begin", d, N, beam, max_len, workspace, workspace_bytes, &w);
   if (rc) return rc;
   if (!embeddings) { set_last_error("sb_decoder_begin: null embeddings"); return SB_ERR_INVALID; }
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
@@ -481,27 +442,16 @@ int sb_decoder_begin(SbDecoder* d, const float* embeddings, int32_t N, int32_t b
   const long long n = (long long)N * D;
   cast_bf16_kernel<<<(unsigned)((n / 4 + 255) / 256 + 1), 256, 0, stream>>>(embeddings, w.ebf, n);
   SB_CUDA_CHECK(cudaGetLastError());
-  GemmArgs g;
-  g.allow_skinny = 1;
-  g.cta_group = 2;
-  g.num_sms = d->num_sms;
-  g.M = N;
-  g.K = D;
-  g.N = D;
-  g.lda = D;
-  g.ldw = D;
-  g.ldc = D;
-  g.residual = nullptr;
-  g.ldr = 0;
-  g.epi = EPI_BIAS;
   for (int li = 0; li < d->cfg.num_layers; ++li) {
     const SbDecoderLayerWeights& L = d->layers[li];
     // v = e Wv^T + bv  (bf16), c = v Wo^T + bo (fp32)
-    g.A = w.ebf; g.W = reinterpret_cast<const __nv_bfloat16*>(L.cross_wv); g.C = w.vtmp; g.out_fp32 = 0; g.bias = L.cross_bv;
-    if ((rc = gemm_bf16(g, stream))) return rc;
-    g.A = w.vtmp; g.W = reinterpret_cast<const __nv_bfloat16*>(L.cross_wo); g.C = w.cross + (size_t)li * N * D; g.out_fp32 = 1;
-    g.bias = L.cross_bo;
-    if ((rc = gemm_bf16(g, stream))) return rc;
+    GemmArgs v = gemm_args(w.ebf, D, L.cross_wv, D, w.vtmp, D, 0, L.cross_bv, N, D, D, EPI_BIAS, d->num_sms);
+    v.allow_skinny = 1;
+    if ((rc = gemm_bf16(v, stream))) return rc;
+    GemmArgs c = gemm_args(w.vtmp, D, L.cross_wo, D, w.cross + (size_t)li * N * D, D, 1, L.cross_bo, N, D, D, EPI_BIAS,
+                           d->num_sms);
+    c.allow_skinny = 1;
+    if ((rc = gemm_bf16(c, stream))) return rc;
   }
   return SB_OK;
 }
@@ -511,7 +461,7 @@ int sb_decoder_step(SbDecoder* d, const int64_t* tokens, const int32_t* table, i
                     const int64_t* probe_tokens, float* out_probe_lprob, void* workspace, size_t workspace_bytes,
                     void* stream_v) {
   DecWs w;
-  int rc = check_ws(d, N, beam, max_len, workspace, workspace_bytes, &w);
+  int rc = check_ws("sb_decoder_step", d, N, beam, max_len, workspace, workspace_bytes, &w);
   if (rc) return rc;
   if (!tokens || !table || !out_lprob || !out_tok || !out_eos_lprob) { set_last_error("sb_decoder_step: null pointer"); return SB_ERR_INVALID; }
   if ((probe_tokens != nullptr) != (out_probe_lprob != nullptr)) {
@@ -529,45 +479,28 @@ int sb_decoder_step(SbDecoder* d, const int64_t* tokens, const int32_t* table, i
                                                       d->cfg.vocab_size, d->pos_table + (size_t)t * D, D,
                                                       d->cfg.embed_scale, w.x, R, w.err_flag);
   SB_CUDA_CHECK(cudaGetLastError());
-  GemmArgs g;
-  g.allow_skinny = 1;
-  g.cta_group = 2;
-  g.num_sms = d->num_sms;
-  g.M = R;
-  g.splitk_flags = w.splitk_flags;  // the residual GEMMs may split K when their tiles leave SM pairs idle (2 560 rows)
-  g.splitk_flags_len = kSplitkFlags;
+  // Every GEMM of a step may take the weight-streaming path; the residual ones may split K when their tiles leave SM
+  // pairs idle (2 560 rows).
+  auto gemm = [&](GemmArgs g) {
+    g.allow_skinny = 1;
+    g.splitk_flags = w.splitk_flags;
+    g.splitk_flags_len = kSplitkFlags;
+    return gemm_bf16(g, stream);
+  };
   const size_t layer_stride = (size_t)R * max_len * D;
   for (int li = 0; li < d->cfg.num_layers; ++li) {
     const SbDecoderLayerWeights& L = d->layers[li];
     if ((rc = layernorm_bf16(w.x, L.ln1_g, L.ln1_b, d->cfg.ln_eps, w.h, R, D, stream))) return rc;
-    g.A = w.h; g.lda = D; g.W = reinterpret_cast<const __nv_bfloat16*>(L.wqkv); g.ldw = D;
-    g.C = w.qkv; g.ldc = 3 * D; g.out_fp32 = 0; g.bias = L.bqkv; g.residual = nullptr; g.ldr = 0;
-    g.N = 3 * D; g.K = D; g.epi = EPI_BIAS;
-    if ((rc = gemm_bf16(g, stream))) return rc;
+    if ((rc = gemm(gemm_args(w.h, D, L.wqkv, D, w.qkv, 3 * D, 0, L.bqkv, R, 3 * D, D, EPI_BIAS, d->num_sms)))) return rc;
     decode_attention_kernel<<<dim3((unsigned)((H + 3) / 4), (unsigned)R), 128, 0, stream>>>(
         w.qkv, w.kcache + li * layer_stride, w.vcache + li * layer_stride, table, t, max_len, H, w.h);
     SB_CUDA_CHECK(cudaGetLastError());
-    g.A = w.h; g.lda = D; g.W = reinterpret_cast<const __nv_bfloat16*>(L.wo); g.ldw = D;
-    g.C = w.x; g.ldc = D; g.out_fp32 = 1; g.bias = L.bo; g.residual = w.x; g.ldr = D;
-    g.N = D; g.K = D; g.epi = EPI_BIAS_RESIDUAL;
-    if ((rc = gemm_bf16(g, stream))) return rc;
-    if (D % 128 == 0 && D <= 128 * kMaxVec) {
-      add_const_layernorm_kernel<<<row_blocks, 256, 0, stream>>>(w.x, w.cross + (size_t)li * N * D, R, beam, D, L.ln3_g,
-                                                                 L.ln3_b, d->cfg.ln_eps, w.h);
-      SB_CUDA_CHECK(cudaGetLastError());
-    } else {
-      add_sentence_const_kernel<<<row_blocks, 256, 0, stream>>>(w.x, w.cross + (size_t)li * N * D, R, beam, D);
-      SB_CUDA_CHECK(cudaGetLastError());
-      if ((rc = layernorm_bf16(w.x, L.ln3_g, L.ln3_b, d->cfg.ln_eps, w.h, R, D, stream))) return rc;
-    }
-    g.A = w.h; g.lda = D; g.W = reinterpret_cast<const __nv_bfloat16*>(L.w1); g.ldw = D;
-    g.C = w.f; g.ldc = F; g.out_fp32 = 0; g.bias = L.b1; g.residual = nullptr; g.ldr = 0;
-    g.N = F; g.K = D; g.epi = EPI_BIAS_RELU;
-    if ((rc = gemm_bf16(g, stream))) return rc;
-    g.A = w.f; g.lda = F; g.W = reinterpret_cast<const __nv_bfloat16*>(L.w2); g.ldw = F;
-    g.C = w.x; g.ldc = D; g.out_fp32 = 1; g.bias = L.b2; g.residual = w.x; g.ldr = D;
-    g.N = D; g.K = F; g.epi = EPI_BIAS_RESIDUAL;
-    if ((rc = gemm_bf16(g, stream))) return rc;
+    if ((rc = gemm(gemm_args(w.h, D, L.wo, D, w.x, D, 1, L.bo, R, D, D, EPI_BIAS_RESIDUAL, d->num_sms)))) return rc;
+    add_const_layernorm_kernel<<<row_blocks, 256, 0, stream>>>(w.x, w.cross + (size_t)li * N * D, R, beam, D, L.ln3_g,
+                                                               L.ln3_b, d->cfg.ln_eps, w.h);
+    SB_CUDA_CHECK(cudaGetLastError());
+    if ((rc = gemm(gemm_args(w.h, D, L.w1, D, w.f, F, 0, L.b1, R, F, D, EPI_BIAS_RELU, d->num_sms)))) return rc;
+    if ((rc = gemm(gemm_args(w.f, F, L.w2, F, w.x, D, 1, L.b2, R, D, F, EPI_BIAS_RESIDUAL, d->num_sms)))) return rc;
   }
   if ((rc = layernorm_bf16(w.x, d->final_ln_g, d->final_ln_b, d->cfg.ln_eps, w.h, R, D, stream))) return rc;
   if ((rc = gemm_bf16_topk(w.h, D, reinterpret_cast<const __nv_bfloat16*>(d->embed), D, R, (int)d->cfg.vocab_size, D,
@@ -583,9 +516,8 @@ int sb_decoder_step(SbDecoder* d, const int64_t* tokens, const int32_t* table, i
 int sb_decoder_check_inputs(SbDecoder* d, void* workspace, void* stream_v) {
   if (!d || !workspace) { set_last_error("sb_decoder_check_inputs: null argument"); return SB_ERR_INVALID; }
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023);
   int32_t flag = 0;
-  SB_CUDA_CHECK(cudaMemcpyAsync(&flag, reinterpret_cast<void*>(base), sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+  SB_CUDA_CHECK(cudaMemcpyAsync(&flag, workspace_base(workspace), sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
   SB_CUDA_CHECK(cudaStreamSynchronize(stream));
   if (flag != 0) {
     set_last_error("token id outside [0, vocab_size) fed to the decoder");

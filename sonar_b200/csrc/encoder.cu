@@ -43,7 +43,22 @@ void set_last_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+int require_hopper(const char* who, int* num_sms) {
+  int n_gpu = 0, dev = 0, major = 0, minor = 0;
+  if (cudaGetDeviceCount(&n_gpu) != cudaSuccess || n_gpu == 0) {
+    set_last_error("%s: no CUDA device (this engine has no CPU path)", who);
+    return SB_ERR_CUDA;
+  }
+  SB_CUDA_CHECK(cudaGetDevice(&dev));
+  SB_CUDA_CHECK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+  SB_CUDA_CHECK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  if (major != 9) {
+    set_last_error("%s: the sm_90a kernels need a Hopper H100-class GPU (found sm_%d%d)", who, major, minor);
+    return SB_ERR_CUDA;
+  }
+  SB_CUDA_CHECK(cudaDeviceGetAttribute(num_sms, cudaDevAttrMultiProcessorCount, dev));
+  return SB_OK;
+}
 
 struct Workspace {
   int32_t* cu;
@@ -93,29 +108,22 @@ struct SbEncoder {
 static Workspace carve(const SbEncoder* e, int32_t max_batch, int64_t max_tokens, void* base) {
   const size_t D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim;
   const size_t T = (size_t)(max_tokens > 0 ? max_tokens : 1);
-  uint8_t* p = reinterpret_cast<uint8_t*>(base);
-  size_t off = 0;
+  Carver c(base);
   Workspace w;
-  w.cu = reinterpret_cast<int32_t*>(p + off);
-  off = align_up(off + sizeof(int32_t) * ((size_t)max_batch + 1), 1024);
-  w.ln_stats = reinterpret_cast<float*>(p + off);
-  off = align_up(off + T * (D / kLnPartCols) * 2 * sizeof(float), 1024);
-  w.x = reinterpret_cast<float*>(p + off);
-  off = align_up(off + T * D * 4, 1024);
-  w.h = reinterpret_cast<__nv_bfloat16*>(p + off);
-  off = align_up(off + T * D * 2, 1024);
-  w.qkv = reinterpret_cast<__nv_bfloat16*>(p + off);
-  off = align_up(off + T * 3 * D * 2, 1024);
-  w.f = reinterpret_cast<__nv_bfloat16*>(p + off);
-  off = align_up(off + T * F * 2, 1024);
-  w.bytes = off;
+  w.cu = c.take<int32_t>(sizeof(int32_t) * ((size_t)max_batch + 1));
+  w.ln_stats = c.take<float>(T * (D / kLnPartCols) * 2 * sizeof(float));
+  w.x = c.take<float>(T * D * 4);
+  w.h = c.take<__nv_bfloat16>(T * D * 2);
+  w.qkv = c.take<__nv_bfloat16>(T * 3 * D * 2);
+  w.f = c.take<__nv_bfloat16>(T * F * 2);
+  w.bytes = c.off;
   return w;
 }
 
 extern "C" {
 
 const char* sb_last_error(void) { return g_err; }
-int sb_version(void) { return 103; }
+int sb_version(void) { return 104; }
 
 int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbEncoder** out) {
   if (!cfg || !w || !out) { set_last_error("sb_encoder_create: null argument"); return SB_ERR_INVALID; }
@@ -131,11 +139,6 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
   }
   if (F <= 0 || F % 256 != 0) { set_last_error("sb_encoder_create: ffn_inner_dim must be a multiple of 256"); return SB_ERR_INVALID; }
   if (cfg->ln_fold < 0 || cfg->ln_fold > 2) { set_last_error("sb_encoder_create: ln_fold must be 0, 1 or 2"); return SB_ERR_INVALID; }
-  if (cfg->epi_groups < 0 || cfg->epi_groups > 2) { set_last_error("sb_encoder_create: epi_groups must be 0, 1 or 2"); return SB_ERR_INVALID; }
-  if (cfg->epi_groups == 1 && (cfg->ln_fold != 0 || cfg->cta_group == 1)) {
-    set_last_error("sb_encoder_create: epi_groups = 1 (the one-warpgroup epilogue kept for A/B runs) needs ln_fold = 0 and paired CTAs");
-    return SB_ERR_INVALID;
-  }
   if (cfg->num_layers < 0 || cfg->pos_rows <= 0 || cfg->vocab_size <= 0) {
     set_last_error("sb_encoder_create: bad num_layers / pos_rows / vocab_size");
     return SB_ERR_INVALID;
@@ -148,19 +151,13 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
     set_last_error("sb_encoder_create: missing weight pointer");
     return SB_ERR_INVALID;
   }
-  int dev = 0, n_gpu = 0;
-  if (cudaGetDeviceCount(&n_gpu) != cudaSuccess || n_gpu == 0) {
-    set_last_error("sb_encoder_create: no CUDA device (this engine has no CPU path)");
-    return SB_ERR_CUDA;
-  }
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  SB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 9) {
-    set_last_error("sb_encoder_create: sm_90a kernels need a Hopper H100-class GPU (found sm_%d%d)", prop.major,
-                   prop.minor);
-    return SB_ERR_CUDA;
-  }
+  for (int i = 0; i < cfg->num_layers; ++i)
+    if (has_null_pointer(w->layers[i])) {
+      set_last_error("sb_encoder_create: layer %d has a null weight pointer", i);
+      return SB_ERR_INVALID;
+    }
+  int num_sms = 0;
+  if (int rc = require_hopper("sb_encoder_create", &num_sms)) return rc;
   SbEncoder* e = new (std::nothrow) SbEncoder();
   if (!e) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   e->cfg = *cfg;
@@ -169,16 +166,7 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
   e->final_ln_g = w->final_ln_g;
   e->final_ln_b = w->final_ln_b;
   e->layers.assign(w->layers, w->layers + cfg->num_layers);
-  for (int i = 0; i < cfg->num_layers; ++i) {
-    const SbLayerWeights& l = e->layers[i];
-    if (!l.wqkv || !l.bqkv || !l.wo || !l.bo || !l.w1 || !l.b1 || !l.w2 || !l.b2 || !l.ln1_g || !l.ln1_b ||
-        !l.ln2_g || !l.ln2_b) {
-      set_last_error("sb_encoder_create: layer %d has a null weight pointer", i);
-      delete e;
-      return SB_ERR_INVALID;
-    }
-  }
-  e->num_sms = cfg->num_sms > 0 ? cfg->num_sms : prop.multiProcessorCount;
+  e->num_sms = cfg->num_sms > 0 ? cfg->num_sms : num_sms;
   for (int i = 0; i < SbEncoder::kSlots; ++i) e->ev_ok[i] = false;
   if (cudaMallocHost(reinterpret_cast<void**>(&e->pinned), sizeof(int32_t) * SbEncoder::kSlots * SbEncoder::kSlotInts) !=
       cudaSuccess) {
@@ -196,25 +184,29 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
     // LayerNorm folding (LnFold): W' = W diag(gamma), c = row sums of W', b' = b + W beta for the two GEMMs that consume a
     // LayerNorm in every layer; prepared once here (the caller's weights are not modified)
     const size_t D_ = D, F_ = F;
-    const size_t per_layer = align_up(3 * D_ * D_ * 2, 256) + align_up(F_ * D_ * 2, 256) + 2 * align_up(3 * D_ * 4, 256) +
-                             2 * align_up(F_ * 4, 256);
-    if (cudaMalloc(&e->fold_pool, per_layer * cfg->num_layers) != cudaSuccess) {
-      set_last_error("sb_encoder_create: cudaMalloc of %zu bytes for the LayerNorm-folded weights failed",
-                     per_layer * cfg->num_layers);
+    auto carve_folded = [&](void* base) {
+      Carver c(base);
+      for (FoldedLayer& f : e->folded) {
+        f.wqkv = c.take<__nv_bfloat16>(3 * D_ * D_ * 2, 256);
+        f.w1 = c.take<__nv_bfloat16>(F_ * D_ * 2, 256);
+        f.cqkv = c.take<float>(3 * D_ * 4, 256);
+        f.bqkv = c.take<float>(3 * D_ * 4, 256);
+        f.c1 = c.take<float>(F_ * 4, 256);
+        f.b1 = c.take<float>(F_ * 4, 256);
+      }
+      return c.off;
+    };
+    e->folded.resize(cfg->num_layers);
+    const size_t pool_bytes = carve_folded(nullptr);
+    if (cudaMalloc(&e->fold_pool, pool_bytes) != cudaSuccess) {
+      set_last_error("sb_encoder_create: cudaMalloc of %zu bytes for the LayerNorm-folded weights failed", pool_bytes);
       sb_encoder_destroy(e);
       return SB_ERR_CUDA;
     }
-    e->folded.resize(cfg->num_layers);
-    uint8_t* p = reinterpret_cast<uint8_t*>(e->fold_pool);
+    carve_folded(e->fold_pool);
     for (int i = 0; i < cfg->num_layers; ++i) {
-      FoldedLayer& f = e->folded[i];
+      const FoldedLayer& f = e->folded[i];
       const SbLayerWeights& l = e->layers[i];
-      f.wqkv = reinterpret_cast<__nv_bfloat16*>(p); p += align_up(3 * D_ * D_ * 2, 256);
-      f.w1 = reinterpret_cast<__nv_bfloat16*>(p); p += align_up(F_ * D_ * 2, 256);
-      f.cqkv = reinterpret_cast<float*>(p); p += align_up(3 * D_ * 4, 256);
-      f.bqkv = reinterpret_cast<float*>(p); p += align_up(3 * D_ * 4, 256);
-      f.c1 = reinterpret_cast<float*>(p); p += align_up(F_ * 4, 256);
-      f.b1 = reinterpret_cast<float*>(p); p += align_up(F_ * 4, 256);
       int rc = fold_layernorm_weights(reinterpret_cast<const __nv_bfloat16*>(l.wqkv), l.bqkv, l.ln1_g, l.ln1_b, 3 * D, D,
                                       f.wqkv, f.cqkv, f.bqkv, nullptr);
       if (!rc)
@@ -255,7 +247,7 @@ int sb_encoder_workspace_bytes(const SbEncoder* enc, int32_t max_batch, int64_t 
     set_last_error("sb_encoder_workspace_bytes: bad argument");
     return SB_ERR_INVALID;
   }
-  *bytes = carve(enc, max_batch, max_tokens, nullptr).bytes + 1024;  // + slack for base alignment
+  *bytes = carve(enc, max_batch, max_tokens, nullptr).bytes + kWorkspaceAlign;
   return SB_OK;
 }
 
@@ -286,13 +278,10 @@ int sb_encoder_forward(SbEncoder* e, const int64_t* ids, int64_t ids_row_stride,
     if (T > 0x7fffffffll) { set_last_error("sb_encoder_forward: too many tokens"); return SB_ERR_INVALID; }
     cu_h[b + 1] = (int32_t)T;
   }
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023);
-  Workspace w = carve(e, B, T, reinterpret_cast<void*>(base));
-  if (base - reinterpret_cast<uintptr_t>(workspace) + w.bytes > workspace_bytes) {
-    set_last_error("sb_encoder_forward: workspace too small (%zu bytes given, %zu needed for B=%d T=%lld)",
-                   workspace_bytes, (size_t)(base - reinterpret_cast<uintptr_t>(workspace)) + w.bytes, B, T);
-    return SB_ERR_INVALID;
-  }
+  Workspace w;
+  int rc = bind_workspace("sb_encoder_forward", workspace, workspace_bytes, &w,
+                          [&](void* p) { return carve(e, B, T, p); });
+  if (rc) return rc;
   SB_CUDA_CHECK(cudaMemcpyAsync(w.cu, cu_h, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice, stream));
   SB_CUDA_CHECK(cudaEventRecord(e->ev[slot], stream));
   if (T == 0) {
@@ -303,77 +292,54 @@ int sb_encoder_forward(SbEncoder* e, const int64_t* ids, int64_t ids_row_stride,
   const bool fold = e->cfg.ln_fold != 0 && e->cfg.num_layers > 0;  // LN1 (attention block) folded into FFN2 -> QKV
   const bool fold2 = fold && e->cfg.ln_fold == 1;                   // LN2 (FFN block) folded into out-proj -> FFN1 as well
   __nv_bfloat16* hn = w.qkv;  // [T, D] view of the (dead after attention) qkv buffer: bf16(x) behind the out-projection
-  int rc;
   if ((rc = embed_tokens(ids, ids_row_stride, w.cu, B, S, reinterpret_cast<const __nv_bfloat16*>(e->embed),
                          e->cfg.vocab_size, e->pos_table, e->cfg.pos_rows, D, e->cfg.embed_scale, w.x, e->err_flag,
                          stream, 0, fold ? w.h : nullptr, fold ? w.ln_stats : nullptr)))
     return rc;
 
-  GemmArgs g;
-  g.cta_group = (e->cfg.cta_group == 1) ? 1 : 2;
-  g.num_sms = e->num_sms;
-  g.M = (int)T;
-  g.epi_groups = (e->cfg.epi_groups == 1) ? 1 : 2;
+  const int cta_group = (e->cfg.cta_group == 1) ? 1 : 2;
+  const int M = (int)T;
   LnFold consume;  // what a LayerNorm-consuming GEMM needs
   consume.stats_in = w.ln_stats;
   consume.chunks = D / kLnPartCols;
   consume.eps = e->cfg.ln_eps;
   for (int li = 0; li < e->cfg.num_layers; ++li) {
     const SbLayerWeights& L = e->layers[li];
+    const FoldedLayer* f = fold ? &e->folded[li] : nullptr;
     // --- self-attention block: x += Wo . SDPA(LN1(x)) + bo ---
     if (!fold)
       if ((rc = layernorm_bf16(w.x, L.ln1_g, L.ln1_b, e->cfg.ln_eps, w.h, T, D, stream))) return rc;
-    g.A = w.h; g.lda = D; g.ldw = D;
-    g.C = w.qkv; g.ldc = 3 * D; g.out_fp32 = 0; g.residual = nullptr; g.ldr = 0;
-    g.N = 3 * D; g.K = D; g.epi = EPI_BIAS;
-    if (fold) {
-      const FoldedLayer& f = e->folded[li];
-      g.W = f.wqkv; g.bias = f.bqkv; g.lf = consume; g.lf.colsum = f.cqkv;
-    } else {
-      g.W = reinterpret_cast<const __nv_bfloat16*>(L.wqkv); g.bias = L.bqkv;
-    }
-    rc = gemm_bf16(g, stream);
-    g.lf = LnFold();
-    if (rc) return rc;
+    GemmArgs qkv = gemm_args(w.h, D, fold ? f->wqkv : L.wqkv, D, w.qkv, 3 * D, 0, fold ? f->bqkv : L.bqkv, M, 3 * D, D,
+                             EPI_BIAS, e->num_sms);
+    qkv.cta_group = cta_group;
+    if (fold) { qkv.lf = consume; qkv.lf.colsum = f->cqkv; }
+    if ((rc = gemm_bf16(qkv, stream))) return rc;
     if ((rc = attention_packed(w.qkv, w.cu, B, H, T, e->num_sms, w.h, stream))) return rc;
-    g.A = w.h; g.lda = D; g.W = reinterpret_cast<const __nv_bfloat16*>(L.wo); g.ldw = D;
-    g.C = w.x; g.ldc = D; g.out_fp32 = 1; g.bias = L.bo; g.residual = w.x; g.ldr = D;
-    g.N = D; g.K = D; g.epi = EPI_BIAS_RESIDUAL;
+    GemmArgs proj = gemm_args(w.h, D, L.wo, D, w.x, D, 1, L.bo, M, D, D, EPI_BIAS_RESIDUAL, e->num_sms);
+    proj.cta_group = cta_group;
     if (fold2) {  // emits x, hn = bf16(x) and the statistics LN2 needs
-      g.epi = EPI_BIAS_RESIDUAL_STATS;
-      g.lf.h_out = hn; g.lf.ldh = D; g.lf.stats_out = w.ln_stats;
+      proj.epi = EPI_BIAS_RESIDUAL_STATS;
+      proj.lf.h_out = hn; proj.lf.ldh = D; proj.lf.stats_out = w.ln_stats;
     }
-    rc = gemm_bf16(g, stream);
-    g.lf = LnFold();
-    if (rc) return rc;
+    if ((rc = gemm_bf16(proj, stream))) return rc;
     // --- feed-forward block: x += W2 . relu(W1 . LN2(x) + b1) + b2 ---
     if (!fold2)
       if ((rc = layernorm_bf16(w.x, L.ln2_g, L.ln2_b, e->cfg.ln_eps, w.h, T, D, stream))) return rc;
-    g.A = fold2 ? hn : w.h; g.lda = D; g.ldw = D;
-    g.C = w.f; g.ldc = F; g.out_fp32 = 0; g.residual = nullptr; g.ldr = 0;
-    g.N = F; g.K = D; g.epi = EPI_BIAS_RELU;
-    if (fold2) {
-      const FoldedLayer& f = e->folded[li];
-      g.W = f.w1; g.bias = f.b1; g.lf = consume; g.lf.colsum = f.c1;
-    } else {
-      g.W = reinterpret_cast<const __nv_bfloat16*>(L.w1); g.bias = L.b1;
-    }
+    GemmArgs ffn1 = gemm_args(fold2 ? hn : w.h, D, fold2 ? f->w1 : L.w1, D, w.f, F, 0, fold2 ? f->b1 : L.b1, M, F, D,
+                              EPI_BIAS_RELU, e->num_sms);
+    ffn1.cta_group = cta_group;
+    if (fold2) { ffn1.lf = consume; ffn1.lf.colsum = f->c1; }
     const bool prof = e->prof_start && li == e->cfg.num_layers / 2;
     if (prof) SB_CUDA_CHECK(cudaEventRecord(e->prof_start, stream));
-    rc = gemm_bf16(g, stream);
-    g.lf = LnFold();
-    if (rc) return rc;
+    if ((rc = gemm_bf16(ffn1, stream))) return rc;
     if (prof) SB_CUDA_CHECK(cudaEventRecord(e->prof_stop, stream));
-    g.A = w.f; g.lda = F; g.W = reinterpret_cast<const __nv_bfloat16*>(L.w2); g.ldw = F;
-    g.C = w.x; g.ldc = D; g.out_fp32 = 1; g.bias = L.b2; g.residual = w.x; g.ldr = D;
-    g.N = D; g.K = F; g.epi = EPI_BIAS_RESIDUAL;
+    GemmArgs ffn2 = gemm_args(w.f, F, L.w2, F, w.x, D, 1, L.b2, M, D, F, EPI_BIAS_RESIDUAL, e->num_sms);
+    ffn2.cta_group = cta_group;
     if (fold && li + 1 < e->cfg.num_layers) {  // emits x, h = bf16(x) and the statistics the next layer's LN1 needs
-      g.epi = EPI_BIAS_RESIDUAL_STATS;
-      g.lf.h_out = w.h; g.lf.ldh = D; g.lf.stats_out = w.ln_stats;
+      ffn2.epi = EPI_BIAS_RESIDUAL_STATS;
+      ffn2.lf.h_out = w.h; ffn2.lf.ldh = D; ffn2.lf.stats_out = w.ln_stats;
     }
-    rc = gemm_bf16(g, stream);
-    g.lf = LnFold();
-    if (rc) return rc;
+    if ((rc = gemm_bf16(ffn2, stream))) return rc;
   }
   return ln_pool(w.x, w.cu, B, D, e->final_ln_g, e->final_ln_b, e->cfg.ln_eps, 1, e->cfg.pooling, out, encoded, S,
                  stream);
@@ -427,17 +393,12 @@ int sb_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void* C
                  const float* bias, const void* residual, int64_t ldr, int32_t M, int32_t N, int32_t K, int32_t epi,
                  int32_t cta_group, void* stream) {
   if (!A || !W || !C) { set_last_error("sb_gemm_bf16: null pointer"); return SB_ERR_INVALID; }
-  GemmArgs g;
-  g.A = reinterpret_cast<const __nv_bfloat16*>(A); g.lda = lda;
-  g.W = reinterpret_cast<const __nv_bfloat16*>(W); g.ldw = ldw;
-  g.C = C; g.ldc = ldc; g.out_fp32 = out_fp32; g.bias = bias; g.residual = residual; g.ldr = ldr;
-  g.M = M; g.N = N; g.K = K; g.epi = epi;
+  int sms = 0;
+  if (int rc = require_hopper("sb_gemm_bf16", &sms)) return rc;
+  GemmArgs g = gemm_args(A, lda, W, ldw, C, ldc, out_fp32, bias, M, N, K, epi, sms);
+  g.residual = residual; g.ldr = ldr;
   g.cta_group = cta_group == 1 ? 1 : 2;
   g.allow_skinny = (cta_group == 0);  // 0 = automatic: M <= 64 may take the weight-streaming path
-  int dev = 0, sms = 0;
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  SB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  g.num_sms = sms;
   return gemm_bf16(g, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -455,52 +416,31 @@ int sb_gemm_ln_consumer(const void* A, int64_t lda, const void* Wf, int64_t ldw,
                         const float* colsum, const float* stats, float eps, int32_t M, int32_t N, int32_t K, int32_t relu,
                         void* stream) {
   if (!A || !Wf || !C || !bias_f || !colsum || !stats) { set_last_error("sb_gemm_ln_consumer: null pointer"); return SB_ERR_INVALID; }
-  GemmArgs g;
-  g.A = reinterpret_cast<const __nv_bfloat16*>(A); g.lda = lda;
-  g.W = reinterpret_cast<const __nv_bfloat16*>(Wf); g.ldw = ldw;
-  g.C = C; g.ldc = ldc; g.out_fp32 = 0; g.bias = bias_f; g.residual = nullptr; g.ldr = 0;
-  g.M = M; g.N = N; g.K = K; g.epi = relu ? EPI_BIAS_RELU : EPI_BIAS;
-  g.cta_group = 2;
+  int sms = 0;
+  if (int rc = require_hopper("sb_gemm_ln_consumer", &sms)) return rc;
+  GemmArgs g = gemm_args(A, lda, Wf, ldw, C, ldc, 0, bias_f, M, N, K, relu ? EPI_BIAS_RELU : EPI_BIAS, sms);
   g.lf.stats_in = stats; g.lf.colsum = colsum; g.lf.chunks = K / kLnPartCols; g.lf.eps = eps;
-  int dev = 0, sms = 0;
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  SB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  g.num_sms = sms;
   return gemm_bf16(g, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int sb_gemm_residual_stats(const void* A, int64_t lda, const void* W, int64_t ldw, float* x, int64_t ldx, const float* bias,
                            void* h_out, int64_t ldh, float* stats_out, int32_t M, int32_t N, int32_t K, void* stream) {
   if (!A || !W || !x || !bias || !h_out || !stats_out) { set_last_error("sb_gemm_residual_stats: null pointer"); return SB_ERR_INVALID; }
-  GemmArgs g;
-  g.A = reinterpret_cast<const __nv_bfloat16*>(A); g.lda = lda;
-  g.W = reinterpret_cast<const __nv_bfloat16*>(W); g.ldw = ldw;
-  g.C = x; g.ldc = ldx; g.out_fp32 = 1; g.bias = bias; g.residual = x; g.ldr = ldx;
-  g.M = M; g.N = N; g.K = K; g.epi = EPI_BIAS_RESIDUAL_STATS;
-  g.cta_group = 2;
+  int sms = 0;
+  if (int rc = require_hopper("sb_gemm_residual_stats", &sms)) return rc;
+  GemmArgs g = gemm_args(A, lda, W, ldw, x, ldx, 1, bias, M, N, K, EPI_BIAS_RESIDUAL_STATS, sms);
   g.lf.h_out = reinterpret_cast<__nv_bfloat16*>(h_out); g.lf.ldh = ldh; g.lf.stats_out = stats_out;
-  int dev = 0, sms = 0;
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  SB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  g.num_sms = sms;
   return gemm_bf16(g, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int sb_gemm_residual_splitk(const void* A, int64_t lda, const void* W, int64_t ldw, float* x, int64_t ldx, const float* bias,
                             int32_t M, int32_t N, int32_t K, int32_t* counters, int64_t n_counters, void* stream) {
   if (!A || !W || !x || !bias || !counters) { set_last_error("sb_gemm_residual_splitk: null pointer"); return SB_ERR_INVALID; }
-  GemmArgs g;
-  g.A = reinterpret_cast<const __nv_bfloat16*>(A); g.lda = lda;
-  g.W = reinterpret_cast<const __nv_bfloat16*>(W); g.ldw = ldw;
-  g.C = x; g.ldc = ldx; g.out_fp32 = 1; g.bias = bias; g.residual = x; g.ldr = ldx;
-  g.M = M; g.N = N; g.K = K; g.epi = EPI_BIAS_RESIDUAL;
-  g.cta_group = 2;
+  int sms = 0;
+  if (int rc = require_hopper("sb_gemm_residual_splitk", &sms)) return rc;
+  GemmArgs g = gemm_args(A, lda, W, ldw, x, ldx, 1, bias, M, N, K, EPI_BIAS_RESIDUAL, sms);
   g.splitk_flags = counters;
   g.splitk_flags_len = n_counters;
-  int dev = 0, sms = 0;
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  SB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  g.num_sms = sms;
   return gemm_bf16(g, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -514,9 +454,8 @@ int sb_layernorm(const float* x, const float* gamma, const float* beta, float ep
 int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t H, int64_t total_tokens, void* out,
                  void* stream) {
   if (!qkv || !cu_seqlens || !out) { set_last_error("sb_attention: null pointer"); return SB_ERR_INVALID; }
-  int dev = 0, sms = 0;
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  SB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms = 0;
+  if (int rc = require_hopper("sb_attention", &sms)) return rc;
   return attention_packed(reinterpret_cast<const __nv_bfloat16*>(qkv), cu_seqlens, B, H, total_tokens, sms,
                           reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<cudaStream_t>(stream));
 }

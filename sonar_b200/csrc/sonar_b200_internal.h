@@ -2,10 +2,13 @@
 // The public C ABI is include/sonar_b200.h.
 #pragma once
 
+#include "../../include/sonar_b200.h"
+
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 namespace sb {
 
@@ -21,6 +24,64 @@ constexpr int kTopkCandidates = 16;  // bf16-similarity candidates per row hande
 enum PoolMode { POOL_MAX = 1, POOL_MEAN = 2, POOL_LAST = 3 };  // = reference `Pooling` enum values (model.py:23-27)
 
 void set_last_error(const char* fmt, ...);
+
+// SM count of the current device in *num_sms, after checking that a device exists and is a Hopper GPU (compute
+// capability 9.x), which the sm_90a kernels need.  SB_ERR_CUDA, with `who` in the message, otherwise.
+int require_hopper(const char* who, int* num_sms);
+
+// True if any pointer of a weight struct made of device pointers only (SbLayerWeights, SbDecoderLayerWeights,
+// SbConformerLayerWeights, SbPoolerLayerWeights) is null.
+template <class Weights>
+bool has_null_pointer(const Weights& w) {
+  static_assert(sizeof(Weights) % sizeof(void*) == 0, "a weight struct holds pointers only");
+  for (size_t i = 0; i < sizeof(Weights) / sizeof(void*); ++i) {
+    const void* p;
+    memcpy(&p, reinterpret_cast<const char*>(&w) + i * sizeof(void*), sizeof(void*));
+    if (!p) return true;
+  }
+  return false;
+}
+
+// ---- workspaces: one caller-owned device buffer per call, carved into the engine's buffers ----
+// Every buffer starts on a kWorkspaceAlign boundary.  The *_workspace_bytes functions add kWorkspaceAlign bytes of slack
+// to the carved size, so that the caller's pointer can be rounded up to that boundary.
+constexpr size_t kWorkspaceAlign = 1024;
+
+inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Bump allocator: take() returns the next buffer and starts the one after it on an `align` boundary.  A null base only
+// sizes the layout; `off` is then the number of bytes it needs.
+struct Carver {
+  uintptr_t base;
+  size_t off = 0;
+  explicit Carver(void* p) : base(reinterpret_cast<uintptr_t>(p)) {}
+  template <class T>
+  T* take(size_t bytes, size_t align = kWorkspaceAlign) {
+    T* p = reinterpret_cast<T*>(base + off);
+    off = align_up(off + bytes, align);
+    return p;
+  }
+};
+
+// Where a workspace's first buffer starts: the caller's pointer rounded up to kWorkspaceAlign.
+inline void* workspace_base(void* workspace) {
+  return reinterpret_cast<void*>((reinterpret_cast<uintptr_t>(workspace) + kWorkspaceAlign - 1) &
+                                 ~uintptr_t(kWorkspaceAlign - 1));
+}
+
+// *ws = carve(workspace_base(workspace)); SB_ERR_INVALID, with `who` in the message, if the layout needs more than the
+// caller's workspace_bytes.
+template <class Layout, class Carve>
+int bind_workspace(const char* who, void* workspace, size_t workspace_bytes, Layout* ws, Carve&& carve) {
+  void* base = workspace_base(workspace);
+  *ws = carve(base);
+  const size_t need = (reinterpret_cast<uintptr_t>(base) - reinterpret_cast<uintptr_t>(workspace)) + ws->bytes;
+  if (need > workspace_bytes) {
+    set_last_error("%s: workspace too small (%zu bytes given, %zu needed)", who, workspace_bytes, need);
+    return SB_ERR_INVALID;
+  }
+  return SB_OK;
+}
 
 // cudaFuncSetAttribute is per device: returns true the first time `flags` (a per-call-site static array of 64 bools)
 // is consulted for the current device.
@@ -61,33 +122,45 @@ inline int device_sm_count() {
 }
 
 struct GemmArgs {
-  const __nv_bfloat16* A;  // [M,K] row-major, ld = lda
-  long long lda;
-  const __nv_bfloat16* W;  // [N,K] row-major (nn.Linear layout), ld = ldw
-  long long ldw;
-  void* C;  // [M,N] bf16 or fp32
-  long long ldc;
-  int out_fp32;
-  const float* bias;     // [N] fp32
-  const void* residual;  // [M,N] same dtype as C (may alias C), ld = ldr
-  long long ldr;
-  int M, N, K;
-  int epi;        // EpiMode
-  int cta_group;  // 1 or 2
-  int num_sms;    // 0 -> device_sm_count()
-  LnFold lf;      // LayerNorm folding (see above); default = off
+  const __nv_bfloat16* A = nullptr;  // [M,K] row-major, ld = lda
+  long long lda = 0;
+  const __nv_bfloat16* W = nullptr;  // [N,K] row-major (nn.Linear layout), ld = ldw
+  long long ldw = 0;
+  void* C = nullptr;  // [M,N] bf16 or fp32
+  long long ldc = 0;
+  int out_fp32 = 0;
+  const float* bias = nullptr;     // [N] fp32
+  const void* residual = nullptr;  // [M,N] same dtype as C (may alias C), ld = ldr
+  long long ldr = 0;
+  int M = 0, N = 0, K = 0;
+  int epi = EPI_BIAS;  // EpiMode
+  int cta_group = 2;   // 1 or 2
+  int num_sms = 0;     // 0 -> device_sm_count()
+  LnFold lf;           // LayerNorm folding (see above); default = off
   // Opt-in to the weight-streaming path for M <= 64 (gemm_skinny.cu).  It sums K in a different order than the wgmma
   // tiles, so a caller that promises results independent of the batch size across the M = 64 boundary (the text
   // encoder: bitwise batch-composition invariance) leaves it off; the decoder step and the speech pooler turn it on.
   int allow_skinny = 0;
-  // accepted for compatibility: the Hopper GEMM has one epilogue schedule
-  int epi_groups = 2;
   // Ordered split-K of the accumulate epilogue (x += A.W^T + b with few tiles): zero-initialised device counters, one per
   // (tile, CTA of the pair, epilogue warpgroup); the kernel leaves them zero.  nullptr = never split.  Changes the
   // summation order (deterministically), so only callers that do not promise batch-size-independent bits pass it.
   int* splitk_flags = nullptr;
   long long splitk_flags_len = 0;
 };
+
+// C = epi(A . W^T + bias) with every option off; the residual epilogues add C itself (x += ...).  Callers set LnFold,
+// split-K counters, the skinny path or a residual other than C on the value returned.
+inline GemmArgs gemm_args(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int out_fp32,
+                          const float* bias, int M, int N, int K, int epi, int num_sms) {
+  GemmArgs g;
+  g.A = static_cast<const __nv_bfloat16*>(A); g.lda = lda;
+  g.W = static_cast<const __nv_bfloat16*>(W); g.ldw = ldw;
+  g.C = C; g.ldc = ldc; g.out_fp32 = out_fp32; g.bias = bias;
+  if (epi == EPI_BIAS_RESIDUAL || epi == EPI_BIAS_RESIDUAL_STATS) { g.residual = C; g.ldr = ldc; }
+  g.M = M; g.N = N; g.K = K; g.epi = epi;
+  g.num_sms = num_sms;
+  return g;
+}
 
 int gemm_bf16(const GemmArgs& g, cudaStream_t stream);
 

@@ -20,8 +20,6 @@
 
 namespace sb {
 
-static inline size_t align_up_sz(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 // one warp per row: y = x / |x| (bf16), norm (fp64)
 __global__ void __launch_bounds__(256)
 l2_normalize_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ xn, double* __restrict__ norm, long long n,
@@ -199,24 +197,23 @@ struct XsimWs {
 };
 
 static XsimWs carve_xsim(int n, int m, int d, void* base) {
-  uint8_t* p = reinterpret_cast<uint8_t*>(base);
-  size_t off = 0;
+  Carver c(base);
   XsimWs w;
-  w.xn = reinterpret_cast<__nv_bfloat16*>(p + off); off = align_up_sz(off + (size_t)n * d * 2, 1024);
-  w.yn = reinterpret_cast<__nv_bfloat16*>(p + off); off = align_up_sz(off + (size_t)m * d * 2, 1024);
-  w.nx = reinterpret_cast<double*>(p + off); off = align_up_sz(off + (size_t)n * 8, 1024);
-  w.ny = reinterpret_cast<double*>(p + off); off = align_up_sz(off + (size_t)m * 8, 1024);
+  w.xn = c.take<__nv_bfloat16>((size_t)n * d * 2);
+  w.yn = c.take<__nv_bfloat16>((size_t)m * d * 2);
+  w.nx = c.take<double>((size_t)n * 8);
+  w.ny = c.take<double>((size_t)m * 8);
   w.chunks = xsim_chunks(n, m);
   const size_t per_row = (size_t)gemm_topk_lists(w.chunks) * kTopkCandidates;
-  w.cand_val = reinterpret_cast<float*>(p + off); off = align_up_sz(off + (size_t)n * per_row * 4, 1024);
-  w.cand_idx = reinterpret_cast<int*>(p + off); off = align_up_sz(off + (size_t)n * per_row * 4, 1024);
+  w.cand_val = c.take<float>((size_t)n * per_row * 4);
+  w.cand_idx = c.take<int>((size_t)n * per_row * 4);
   w.merged_val = nullptr;
   w.merged_idx = nullptr;
   if (w.chunks > 1) {
-    w.merged_val = reinterpret_cast<float*>(p + off); off = align_up_sz(off + (size_t)n * 32 * 4, 1024);
-    w.merged_idx = reinterpret_cast<int*>(p + off); off = align_up_sz(off + (size_t)n * 32 * 4, 1024);
+    w.merged_val = c.take<float>((size_t)n * 32 * 4);
+    w.merged_idx = c.take<int>((size_t)n * 32 * 4);
   }
-  w.bytes = off;
+  w.bytes = c.off;
   return w;
 }
 
@@ -369,17 +366,17 @@ struct XsimBidirWs {
 static XsimBidirWs carve_xsim_bidir(int n, int m, int d, void* base) {
   XsimBidirWs w;
   w.base = carve_xsim(n, m, d, base);
-  uint8_t* p = reinterpret_cast<uint8_t*>(base);
-  size_t off = w.base.bytes;
+  Carver c(base);
+  c.off = w.base.bytes;  // the reverse direction's buffers follow the forward layout
   const size_t mp = ((size_t)m + 255) / 256 * 256;
-  w.s_val = reinterpret_cast<float*>(p + off); off = align_up_sz(off + (size_t)m * kXsimCands * 4, 1024);
-  w.s_idx = reinterpret_cast<int*>(p + off); off = align_up_sz(off + (size_t)m * kXsimCands * 4, 1024);
-  w.thr = reinterpret_cast<float*>(p + off); off = align_up_sz(off + mp * 4, 1024);
-  w.thr8 = reinterpret_cast<float*>(p + off); off = align_up_sz(off + mp / 8 * 4, 1024);
-  w.cnt = reinterpret_cast<int*>(p + off); off = align_up_sz(off + (size_t)m * 4, 1024);
-  w.overflow = reinterpret_cast<int*>(p + off); off = align_up_sz(off + 256, 1024);
-  w.buf = reinterpret_cast<uint2*>(p + off); off = align_up_sz(off + (size_t)m * kColCap * 8, 1024);
-  w.bytes = off;
+  w.s_val = c.take<float>((size_t)m * kXsimCands * 4);
+  w.s_idx = c.take<int>((size_t)m * kXsimCands * 4);
+  w.thr = c.take<float>(mp * 4);
+  w.thr8 = c.take<float>(mp / 8 * 4);
+  w.cnt = c.take<int>((size_t)m * 4);
+  w.overflow = c.take<int>(256);
+  w.buf = c.take<uint2>((size_t)m * kColCap * 8);
+  w.bytes = c.off;
   return w;
 }
 }  // namespace sb
@@ -390,7 +387,7 @@ extern "C" {
 
 int sb_xsim_workspace_bytes(int32_t n, int32_t m, int32_t d, size_t* bytes) {
   if (n <= 0 || m <= 0 || d <= 0 || !bytes) { set_last_error("sb_xsim_workspace_bytes: bad argument"); return SB_ERR_INVALID; }
-  *bytes = carve_xsim(n, m, d, nullptr).bytes + 1024;
+  *bytes = carve_xsim(n, m, d, nullptr).bytes + kWorkspaceAlign;
   return SB_OK;
 }
 
@@ -401,20 +398,16 @@ int sb_xsim_knn(const float* x, const float* y, int32_t n, int32_t m, int32_t d,
   if (d <= 0 || d % 64 != 0) { set_last_error("sb_xsim_knn: embedding dim must be a multiple of 64 (got %d)", d); return SB_ERR_INVALID; }
   if (k <= 0 || k > kTopkCandidates) { set_last_error("sb_xsim_knn: k must be in [1, %d]", kTopkCandidates); return SB_ERR_INVALID; }
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023);
-  XsimWs w = carve_xsim(n, m, d, reinterpret_cast<void*>(base));
-  if (base - reinterpret_cast<uintptr_t>(workspace) + w.bytes > workspace_bytes) {
-    set_last_error("sb_xsim_knn: workspace too small");
-    return SB_ERR_INVALID;
-  }
-  int dev = 0, sms = 0;
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  SB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  XsimWs w;
+  int rc = bind_workspace("sb_xsim_knn", workspace, workspace_bytes, &w, [&](void* p) { return carve_xsim(n, m, d, p); });
+  if (rc) return rc;
+  int sms = 0;
+  if ((rc = require_hopper("sb_xsim_knn", &sms))) return rc;
   l2_normalize_kernel<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(x, w.xn, w.nx, n, d);
   l2_normalize_kernel<<<(unsigned)((m + 7) / 8), 256, 0, stream>>>(y, w.yn, w.ny, m, d);
   SB_CUDA_CHECK(cudaGetLastError());
-  int rc = gemm_bf16_topk(w.xn, d, w.yn, d, n, m, d, w.cand_val, w.cand_idx, nullptr, w.chunks, 2, sms, stream);
-  if (rc) return rc;
+  if ((rc = gemm_bf16_topk(w.xn, d, w.yn, d, n, m, d, w.cand_val, w.cand_idx, nullptr, w.chunks, 2, sms, stream)))
+    return rc;
   const float* cv = w.cand_val;
   const int* ci = w.cand_idx;
   if (w.chunks > 1) {
@@ -433,7 +426,7 @@ int sb_xsim_knn(const float* x, const float* y, int32_t n, int32_t m, int32_t d,
 
 int sb_xsim_bidir_workspace_bytes(int32_t n, int32_t m, int32_t d, size_t* bytes) {
   if (n <= 0 || m <= 0 || d <= 0 || !bytes) { set_last_error("sb_xsim_bidir_workspace_bytes: bad argument"); return SB_ERR_INVALID; }
-  *bytes = carve_xsim_bidir(n, m, d, nullptr).bytes + 1024;
+  *bytes = carve_xsim_bidir(n, m, d, nullptr).bytes + kWorkspaceAlign;
   return SB_OK;
 }
 
@@ -448,24 +441,21 @@ int sb_xsim_knn_bidir(const float* x, const float* y, int32_t n, int32_t m, int3
   if (d <= 0 || d % 64 != 0) { set_last_error("sb_xsim_knn_bidir: embedding dim must be a multiple of 64 (got %d)", d); return SB_ERR_INVALID; }
   if (k <= 0 || k > kTopkCandidates) { set_last_error("sb_xsim_knn_bidir: k must be in [1, %d]", kTopkCandidates); return SB_ERR_INVALID; }
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023);
-  XsimBidirWs w = carve_xsim_bidir(n, m, d, reinterpret_cast<void*>(base));
-  if (base - reinterpret_cast<uintptr_t>(workspace) + w.bytes > workspace_bytes) {
-    set_last_error("sb_xsim_knn_bidir: workspace too small");
-    return SB_ERR_INVALID;
-  }
-  int dev = 0, sms = 0;
-  SB_CUDA_CHECK(cudaGetDevice(&dev));
-  SB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  XsimBidirWs w;
+  int rc = bind_workspace("sb_xsim_knn_bidir", workspace, workspace_bytes, &w,
+                          [&](void* p) { return carve_xsim_bidir(n, m, d, p); });
+  if (rc) return rc;
+  int sms = 0;
+  if ((rc = require_hopper("sb_xsim_knn_bidir", &sms))) return rc;
   l2_normalize_kernel<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(x, w.base.xn, w.base.nx, n, d);
   l2_normalize_kernel<<<(unsigned)((m + 7) / 8), 256, 0, stream>>>(y, w.base.yn, w.base.ny, m, d);
   SB_CUDA_CHECK(cudaGetLastError());
   // (1) thresholds of the y rows from a strided sample of the x rows: y^ . xs^T with the usual running top-16 per row
   const int stride = n >= 512 * kSampleStride ? kSampleStride : (n >= 1024 ? n / 512 : 1);
   const int ns = (n + stride - 1) / stride;
-  int rc = gemm_bf16_topk(w.base.yn, d, w.base.xn, (long long)stride * d, m, ns, d, w.s_val, w.s_idx, nullptr, 1, 2, sms,
-                          stream);
-  if (rc) return rc;
+  if ((rc = gemm_bf16_topk(w.base.yn, d, w.base.xn, (long long)stride * d, m, ns, d, w.s_val, w.s_idx, nullptr, 1, 2, sms,
+                           stream)))
+    return rc;
   const long long mp = ((long long)m + 255) / 256 * 256;
   fill_f32_kernel<<<(unsigned)((mp + 255) / 256), 256, 0, stream>>>(w.thr, mp, INFINITY);  // padding columns: never hit
   col_threshold_kernel<<<(unsigned)((m + 7) / 8), 256, 0, stream>>>(w.s_val, w.s_idx, gemm_topk_lists(1), m, w.thr);

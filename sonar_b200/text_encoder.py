@@ -139,18 +139,13 @@ class B200TextEncoderModel(torch.nn.Module):
     """SONAR text encoder (24-layer pre-LN Transformer + final LN + pooling) on sm_90a kernels."""
 
     def __init__(self, config: SonarTextEncoderConfig, state_dict: Dict[str, Tensor],
-                 device: Union[str, torch.device] = "cuda", *, cta_group: int = 2, ln_fold: Union[bool, int] = False,
-                 epi_groups: Optional[int] = None) -> None:
+                 device: Union[str, torch.device] = "cuda", *, cta_group: int = 2,
+                 ln_fold: Union[bool, int] = False) -> None:
         """``ln_fold=True``: the engine folds every encoder-layer LayerNorm into the GEMMs around it (see
         ``SbEncoderConfig.ln_fold`` in ``include/sonar_b200.h``); the default runs the separate LayerNorm kernels
-        (``bench.py`` A/Bs the schedules in every run, ``ab_schedule_variants``).  ``epi_groups`` is kept for callers that pass
-        it: the Hopper GEMM has one epilogue schedule (its two MMA warpgroups run it), so 1 and 2 select the same kernel;
-        ``None`` means 1 without and 2 with ``ln_fold``."""
+        (``bench.py`` A/Bs the schedules in every run, ``ab_schedule_variants``)."""
         super().__init__()
-        if epi_groups is None:
-            epi_groups = 2 if int(ln_fold) else 1
         self.ln_fold = int(ln_fold)  # 0 = separate LayerNorm kernels, 1 = both folded, 2 = only the attention-block one
-        self.epi_groups = int(epi_groups)
         _check_supported(config)
         self.config = config
         self.model_dim = config.model_dim
@@ -203,7 +198,7 @@ class B200TextEncoderModel(torch.nn.Module):
             model_dim=d, num_layers=L, num_heads=config.num_encoder_attn_heads, ffn_inner_dim=config.ffn_inner_dim,
             vocab_size=config.vocab_info.size, pos_rows=max_len, pooling=self.pooling.value, ln_eps=1e-5,
             embed_scale=1.0 if config.no_scale_embedding else math.sqrt(d), cta_group=cta_group, num_sms=0,
-            ln_fold=int(ln_fold), epi_groups=int(epi_groups))
+            ln_fold=int(ln_fold))
         layers_c = (_lib.SbLayerWeights * max(L, 1))()
         for i, bufs in enumerate(self._layer_bufs):
             for k, v in bufs.items():

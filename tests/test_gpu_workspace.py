@@ -1,0 +1,77 @@
+"""Every C-ABI entry point that carves the caller's workspace rejects one that is too small (SB_ERR_INVALID, a message that
+names the entry point) instead of writing past its end.  Engines are the small configurations of the other GPU tests."""
+
+import ctypes as C
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+VOCAB = 4096
+
+
+@pytest.fixture(scope="module")
+def engines(native_lib, cuda_device):
+    from oracle.speech_encoder import OracleSpeechConfig, make_synthetic_speech_state_dict
+    from oracle.text_decoder import OracleDecoderConfig, make_synthetic_decoder_state_dict
+    from oracle.text_encoder import OracleEncoderConfig, make_synthetic_state_dict
+    from sonar_b200 import (B200SpeechEncoderModel, B200TextDecoderModel, B200TextEncoderModel, VocabularyInfo,
+                            sonar_speech_encoder_config, sonar_text_decoder_config, sonar_text_encoder_config)
+
+    vocab = VocabularyInfo(size=VOCAB, unk_idx=1, bos_idx=2, eos_idx=3, pad_idx=1)
+    enc_sd = make_synthetic_state_dict(OracleEncoderConfig(vocab_size=VOCAB, num_layers=2), seed=1)
+    encoder = B200TextEncoderModel(sonar_text_encoder_config("basic", num_encoder_layers=2, vocab_info=vocab), enc_sd,
+                                   cuda_device)
+    dec_sd = make_synthetic_decoder_state_dict(OracleDecoderConfig(vocab_size=VOCAB, num_layers=2, max_seq_len=64), seed=2)
+    decoder = B200TextDecoderModel(sonar_text_decoder_config("basic", num_decoder_layers=2, max_seq_len=64,
+                                                             vocab_info=vocab), dec_sd, cuda_device)
+    sp_sd = make_synthetic_speech_state_dict(OracleSpeechConfig(num_layers=2, pooler_layers=2), seed=3)
+    speech = B200SpeechEncoderModel(sonar_speech_encoder_config("english", num_encoder_layers=2, num_decoder_layers=2),
+                                    sp_sd, cuda_device)
+    return encoder, decoder, speech
+
+
+def test_too_small_workspace_is_rejected(engines, cuda_device):
+    from sonar_b200 import _lib
+
+    encoder, decoder, speech = engines
+    lib = encoder._lib
+    dev = cuda_device
+    bufs = []
+
+    def t(*shape, dtype=torch.float32):
+        bufs.append(torch.zeros(shape, dtype=dtype, device=dev))
+        return bufs[-1].data_ptr()
+
+    w, stream = t(1, dtype=torch.uint8), torch.cuda.current_stream(dev).cuda_stream
+    B, S, D = 4, 16, 1024                 # text / speech batch
+    n, beam, max_len = 3, 2, 16           # decoder: sentences x beam hypotheses
+    R = n * beam
+    lens = (C.c_int32 * B)(*[8] * B)      # 8 speech positions per utterance (16 fbank frames)
+    rows = 256                            # relative-position table rows for 8 positions: roundup(2 * 8 - 1, 256)
+    cu = torch.arange(0, 8 * (B + 1), 8, dtype=torch.int32, device=dev)
+    x, y = t(256, 64), t(512, 64)         # xsim: 256 x 512 rows of dimension 64
+    calls = {
+        "sb_encoder_forward": lambda: lib.sb_encoder_forward(
+            encoder._handle, t(B, S, dtype=torch.int64), S, None, B, S, t(B, D), None, w, 1, stream),
+        "sb_decoder_begin": lambda: lib.sb_decoder_begin(decoder._handle, t(n, D), n, beam, max_len, w, 1, stream),
+        "sb_decoder_step": lambda: lib.sb_decoder_step(
+            decoder._handle, t(R, dtype=torch.int64), t(R, max_len, dtype=torch.int32), 0, n, beam, max_len, t(R, 16),
+            t(R, 16, dtype=torch.int32), t(R), None, None, w, 1, stream),
+        "sb_speech_encoder_forward": lambda: lib.sb_speech_encoder_forward(
+            speech._handle, t(B, 2 * 8, 80), 2 * 8, cu.data_ptr(), lens, B, t(rows, D, dtype=torch.bfloat16), rows,
+            t(B, D), None, w, 1, stream),
+        "sb_xsim_knn": lambda: lib.sb_xsim_knn(
+            x, y, 256, 512, 64, 4, t(256, 4, dtype=torch.float64), t(256, 4, dtype=torch.int32), w, 1, stream),
+        "sb_xsim_knn_bidir": lambda: lib.sb_xsim_knn_bidir(
+            x, y, 256, 512, 64, 4, t(256, 4, dtype=torch.float64), t(256, 4, dtype=torch.int32),
+            t(512, 4, dtype=torch.float64), t(512, 4, dtype=torch.int32), t(1, dtype=torch.int32), w, 1, stream),
+    }
+    for name, call in calls.items():
+        with torch.cuda.device(dev):
+            rc = call()
+        msg = _lib.last_error()
+        assert rc == _lib.SB_ERR_INVALID, (name, rc, msg)
+        assert msg.startswith(f"{name}: workspace too small"), (name, msg)
+    torch.cuda.synchronize(dev)
