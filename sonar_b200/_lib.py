@@ -62,20 +62,17 @@ class SbSpeechConfig(C.Structure):
                 ("pooler_ffn_inner_dim", C.c_int32), ("ln_eps", C.c_float), ("attn_impl", C.c_int32)]
 
 
-CONFORMER_FIELDS = ("ffn1_ln_g", "ffn1_ln_b", "ffn1_w1", "ffn1_b1", "ffn1_w2", "ffn1_b2", "attn_ln_g", "attn_ln_b",
-                    "wqkv", "bqkv", "wo", "bo", "wr", "u_bias", "v_bias", "conv_ln_g", "conv_ln_b", "pw1", "dw",
-                    "bn_scale", "bn_shift", "pw2", "ffn2_ln_g", "ffn2_ln_b", "ffn2_w1", "ffn2_b1", "ffn2_w2", "ffn2_b2",
-                    "ln_g", "ln_b")
-POOLER_FIELDS = ("sa_wv", "sa_bv", "sa_wo", "sa_bo", "sa_ln_g", "sa_ln_b", "ca_wq", "ca_bq", "ca_wkv", "ca_bkv",
-                 "ca_wo", "ca_bo", "ca_ln_g", "ca_ln_b", "w1", "b1", "w2", "b2", "ffn_ln_g", "ffn_ln_b")
-
-
 class SbConformerLayerWeights(C.Structure):
-    _fields_ = [(n, C.c_void_p) for n in CONFORMER_FIELDS]
+    _fields_ = [(n, C.c_void_p) for n in (
+        "ffn1_ln_g", "ffn1_ln_b", "ffn1_w1", "ffn1_b1", "ffn1_w2", "ffn1_b2", "attn_ln_g", "attn_ln_b", "wqkv", "bqkv",
+        "wo", "bo", "wr", "u_bias", "v_bias", "conv_ln_g", "conv_ln_b", "pw1", "dw", "bn_scale", "bn_shift", "pw2",
+        "ffn2_ln_g", "ffn2_ln_b", "ffn2_w1", "ffn2_b1", "ffn2_w2", "ffn2_b2", "ln_g", "ln_b")]
 
 
 class SbPoolerLayerWeights(C.Structure):
-    _fields_ = [(n, C.c_void_p) for n in POOLER_FIELDS]
+    _fields_ = [(n, C.c_void_p) for n in (
+        "sa_wv", "sa_bv", "sa_wo", "sa_bo", "sa_ln_g", "sa_ln_b", "ca_wq", "ca_bq", "ca_wkv", "ca_bkv", "ca_wo", "ca_bo",
+        "ca_ln_g", "ca_ln_b", "w1", "b1", "w2", "b2", "ffn_ln_g", "ffn_ln_b")]
 
 
 class SbSpeechWeights(C.Structure):
@@ -174,6 +171,14 @@ def load() -> C.CDLL:
 def last_error() -> str:
     msg = load().sb_last_error()
     return msg.decode("utf-8", "replace") if msg else ""
+
+
+def workspace_bytes(query, *args) -> int:
+    """Bytes the ``sb_*_workspace_bytes`` entry point ``query`` (a function of the loaded library) asks for; ``args``
+    are its arguments before the out-pointer."""
+    need = C.c_size_t()
+    check(query(*args, C.byref(need)), query.__name__)
+    return need.value
 
 
 def check(rc: int, what: str) -> None:

@@ -20,7 +20,7 @@ POOLING_MODES = {"max": _lib.SB_POOL_MAX, "mean": _lib.SB_POOL_MEAN, "last": _li
 def _need_cuda(*tensors: Optional[Tensor]) -> None:
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("sonar_b200 ops run on CUDA tensors only (no CPU fallback exists)")
+            raise RuntimeError("sonar_b200 runs on CUDA tensors only (no CPU fallback exists)")
 
 
 def _stream() -> int:
@@ -88,7 +88,7 @@ def fold_layernorm(w: Tensor, bias: Tensor, gamma: Tensor, beta: Tensor):
 
 def gemm_residual_stats(a: Tensor, w: Tensor, bias: Tensor, x: Tensor):
     """x += a . w^T + bias in place (fp32); -> (h = bf16(x) [M,N], stats fp32 [M, N/128, 2]): partial 2*t + g holds (mean, M2)
-    of the 128 columns {256 t + 32 c + j : c % 2 == g, j < 32} of the new row (epilogue warpgroup g's share of tile t)."""
+    of column half g of 256-column tile t of the new row, i.e. of columns 256 t + 128 g ... 256 t + 128 g + 127."""
     _need_cuda(a, w, bias, x)
     m, k = a.shape
     n = w.shape[0]

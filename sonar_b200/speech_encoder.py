@@ -10,14 +10,16 @@ arithmetic is in ``sb_speech_encoder_forward`` (``csrc/conformer.cu``).
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import math
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Union
+from typing import Dict, Optional, Union
 
 import torch
 from torch import Tensor
 
 from . import _lib
+from ._engine import EngineModel
 from .sequence import PaddingMask, SequenceBatch, SonarEncoderOutput
 
 
@@ -48,11 +50,7 @@ def sonar_speech_encoder_config(arch: str = "english", **overrides) -> SonarSpee
         cfg = SonarSpeechEncoderConfig(num_decoder_layers=6)
     else:
         raise ValueError(f"unknown sonar speech encoder arch {arch!r}")
-    for k, v in overrides.items():
-        if not hasattr(cfg, k):
-            raise TypeError(f"unknown config field {k!r}")
-        setattr(cfg, k, v)
-    return cfg
+    return dataclasses.replace(cfg, **overrides)
 
 
 def relative_position_table(max_len: int, dim: int, rows: int) -> Tensor:
@@ -69,44 +67,31 @@ def relative_position_table(max_len: int, dim: int, rows: int) -> Tensor:
     return out
 
 
-class B200SpeechEncoderModel(torch.nn.Module):
+class B200SpeechEncoderModel(EngineModel):
+    _abi = "speech_encoder"
+    _default_config = staticmethod(sonar_speech_encoder_config)
+
     def __init__(self, config: SonarSpeechEncoderConfig, state_dict: Dict[str, Tensor],
                  device: Union[str, torch.device] = "cuda", *, attn_impl: str = "mma_sync") -> None:
         """``attn_impl``: relative-position attention kernel -- "mma_sync" (default; the two have not been timed against each
         other on the H100) or "tcgen05" (the name the wgmma kernel keeps)
         (``csrc/attention_relpos_tc.cu``: band product, Q K^T and P V on the tensor cores (wgmma), bitwise independent of the
         batch an utterance is in; ``bench.py`` times both in its speech block)."""
-        super().__init__()
+        super().__init__(device)
         if attn_impl not in ("tcgen05", "mma_sync"):
             raise ValueError("attn_impl must be 'tcgen05' or 'mma_sync'")
         self.attn_impl = attn_impl
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise RuntimeError("B200SpeechEncoderModel needs a CUDA device (there is no CPU path)")
-        if dev.index is None:
-            dev = torch.device("cuda", torch.cuda.current_device())
-        self.device, self.config, self.model_dim = dev, config, config.model_dim
-        self._lib = _lib.load()
+        self.config, self.model_dim = config, config.model_dim
         sd, d = state_dict, config.model_dim
-        keep: List[Tensor] = []
+        bf, f32 = self._bf16, self._f32
 
-        def bf(t):
-            t = t.detach().to(device=dev, dtype=torch.bfloat16).contiguous()
-            keep.append(t)
-            return t
-
-        def f32(t):
-            t = t.detach().to(device=dev, dtype=torch.float32).contiguous()
-            keep.append(t)
-            return t
-
-        layers_c = (_lib.SbConformerLayerWeights * max(config.num_encoder_layers, 1))()
+        layers, pooler = [], []
         for i in range(config.num_encoder_layers):
             p = f"encoder.layers.{i}."
             a = p + "self_attn."
             bn = p + "conv.batch_norm."
             scale = sd[bn + "weight"].float() / torch.sqrt(sd[bn + "running_var"].float() + config.bn_eps)
-            vals = {
+            layers.append({
                 "ffn1_ln_g": f32(sd[p + "ffn1_layer_norm.weight"]), "ffn1_ln_b": f32(sd[p + "ffn1_layer_norm.bias"]),
                 "ffn1_w1": bf(sd[p + "ffn1.inner_proj.weight"]), "ffn1_b1": f32(sd[p + "ffn1.inner_proj.bias"]),
                 "ffn1_w2": bf(sd[p + "ffn1.output_proj.weight"].float() * 0.5), "ffn1_b2": f32(sd[p + "ffn1.output_proj.bias"].float() * 0.5),
@@ -125,14 +110,11 @@ class B200SpeechEncoderModel(torch.nn.Module):
                 "ffn2_w1": bf(sd[p + "ffn2.inner_proj.weight"]), "ffn2_b1": f32(sd[p + "ffn2.inner_proj.bias"]),
                 "ffn2_w2": bf(sd[p + "ffn2.output_proj.weight"].float() * 0.5), "ffn2_b2": f32(sd[p + "ffn2.output_proj.bias"].float() * 0.5),
                 "ln_g": f32(sd[p + "layer_norm.weight"]), "ln_b": f32(sd[p + "layer_norm.bias"]),
-            }
-            for k in _lib.CONFORMER_FIELDS:
-                setattr(layers_c[i], k, vals[k].data_ptr())
-        pool_c = (_lib.SbPoolerLayerWeights * max(config.num_decoder_layers, 1))()
+            })
         for i in range(config.num_decoder_layers):
             p = f"encoder_pooler.decoder.layers.{i}."
             s_, c_ = p + "self_attn.", p + "encoder_decoder_attn."
-            vals = {
+            pooler.append({
                 "sa_wv": bf(sd[s_ + "v_proj.weight"]), "sa_bv": f32(sd[s_ + "v_proj.bias"]),
                 "sa_wo": bf(sd[s_ + "output_proj.weight"]), "sa_bo": f32(sd[s_ + "output_proj.bias"]),
                 "sa_ln_g": f32(sd[p + "self_attn_layer_norm.weight"]), "sa_ln_b": f32(sd[p + "self_attn_layer_norm.bias"]),
@@ -145,9 +127,7 @@ class B200SpeechEncoderModel(torch.nn.Module):
                 "w1": bf(sd[p + "ffn.inner_proj.weight"]), "b1": f32(sd[p + "ffn.inner_proj.bias"]),
                 "w2": bf(sd[p + "ffn.output_proj.weight"]), "b2": f32(sd[p + "ffn.output_proj.bias"]),
                 "ffn_ln_g": f32(sd[p + "ffn_layer_norm.weight"]), "ffn_ln_b": f32(sd[p + "ffn_layer_norm.bias"]),
-            }
-            for k in _lib.POOLER_FIELDS:
-                setattr(pool_c[i], k, vals[k].data_ptr())
+            })
         fw = torch.zeros((d, 192), dtype=torch.float32)
         fw[:, : config.feature_dim] = sd["encoder_frontend.model_dim_proj.weight"].float()
         # TransformerEmbeddingFrontend(embed, SinusoidalPositionEncoder): E[bos] * sqrt(d) + pos[0] = [0.. | 1..]  [fs2]
@@ -161,47 +141,24 @@ class B200SpeechEncoderModel(torch.nn.Module):
             "pooler_q0": f32(q0), "proj_w": bf(sd["encoder_pooler.projection_out.weight"]),
             "zeros": f32(torch.zeros(8192)),
         }
-        w_c = _lib.SbSpeechWeights(layers=layers_c, pooler=pool_c, **{k: v.data_ptr() for k, v in top.items()})
+        w_c = _lib.SbSpeechWeights(layers=self._layer_array(_lib.SbConformerLayerWeights, layers),
+                                   pooler=self._layer_array(_lib.SbPoolerLayerWeights, pooler),
+                                   **{k: v.data_ptr() for k, v in top.items()})
         cfg_c = _lib.SbSpeechConfig(model_dim=d, num_layers=config.num_encoder_layers, num_heads=config.num_encoder_attn_heads,
                                     ffn_inner_dim=config.ffn_inner_dim, conv_kernel=config.depthwise_conv_kernel_size,
                                     pooler_layers=config.num_decoder_layers,
                                     pooler_ffn_inner_dim=config.decoder_ffn_inner_dim, ln_eps=1e-5,
                                     attn_impl=1 if attn_impl == "mma_sync" else 0)
-        handle = C.c_void_p()
-        with torch.cuda.device(dev):
-            _lib.check(self._lib.sb_speech_encoder_create(C.byref(cfg_c), C.byref(w_c), C.byref(handle)),
-                       "sb_speech_encoder_create")
-        self._handle, self._keep = handle, keep
-        self._workspace: Optional[Tensor] = None
+        self._create(cfg_c, w_c)
         self._relpos: Dict[int, Tensor] = {}
         self.return_encoded_seqs = False
-
-    @classmethod
-    def from_checkpoint(cls, path, config: Optional["SonarSpeechEncoderConfig"] = None,
-                        device: Union[str, torch.device] = "cuda") -> "B200SpeechEncoderModel":
-        """Load a fairseq2-layout checkpoint ``{"model": state_dict}`` (key names of ``sonar_speech/handler.py:63-110``)."""
-        ckpt = torch.load(str(path), map_location="cpu", weights_only=True)
-        sd = ckpt["model"] if "model" in ckpt else ckpt
-        return cls(config or sonar_speech_encoder_config("english"), sd, device)
-
-    @property
-    def dtype(self) -> torch.dtype:
-        return torch.bfloat16
-
-    def __del__(self) -> None:  # pragma: no cover
-        try:
-            if getattr(self, "_handle", None):
-                self._lib.sb_speech_encoder_destroy(self._handle)
-                self._handle = None
-        except Exception:
-            pass
 
     @torch.inference_mode()
     def forward(self, batch: SequenceBatch) -> SonarEncoderOutput:
         fb = batch.seqs
         if fb.dim() != 3 or fb.shape[2] != 80:
             raise ValueError("expected fbank features of shape [N, T, 80]")
-        fb = fb.to(device=self.device, dtype=torch.float32).contiguous()
+        fb = self._on_device(fb, torch.float32).contiguous()
         n, t, _ = fb.shape
         frames = batch.padding_mask.seq_lens_host if batch.padding_mask is not None else [t] * n
         lens = [f // 2 for f in frames]  # Wav2Vec2FbankFeatureExtractor stride 2: seq_len // 2 (App. B.2)
@@ -217,19 +174,13 @@ class B200SpeechEncoderModel(torch.nn.Module):
         cu = torch.zeros(n + 1, dtype=torch.int32)
         cu[1:] = torch.cumsum(torch.tensor(lens), 0).to(torch.int32)
         cu_d = cu.to(self.device)
-        need = C.c_size_t()
-        _lib.check(self._lib.sb_speech_encoder_workspace_bytes(self._handle, n, total, smax, C.byref(need)),
-                   "sb_speech_encoder_workspace_bytes")
-        if self._workspace is None or self._workspace.numel() < need.value:
-            self._workspace = None
-            self._workspace = torch.empty(need.value + 4096, dtype=torch.uint8, device=self.device)
+        ws = self._ensure_workspace(n, total, smax)
         out = torch.empty((n, self.model_dim), dtype=torch.float32, device=self.device)
         enc = torch.empty((total, self.model_dim), dtype=torch.float32, device=self.device) if self.return_encoded_seqs else None
         lens_c = (C.c_int32 * n)(*lens)
         with torch.cuda.device(self.device):
             rc = self._lib.sb_speech_encoder_forward(
                 self._handle, fb.data_ptr(), t, cu_d.data_ptr(), lens_c, n, rel.data_ptr(), rows, out.data_ptr(),
-                enc.data_ptr() if enc is not None else None, self._workspace.data_ptr(), self._workspace.numel(),
-                torch.cuda.current_stream(self.device).cuda_stream)
+                enc.data_ptr() if enc is not None else None, ws.data_ptr(), ws.numel(), self._stream())
         _lib.check(rc, "sb_speech_encoder_forward")
         return SonarEncoderOutput(encoded_seqs=enc, sentence_embeddings=out, padding_mask=batch.padding_mask)

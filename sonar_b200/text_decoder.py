@@ -11,17 +11,17 @@ returns the 16 most probable next tokens per hypothesis (log-softmax over the fu
 
 from __future__ import annotations
 
-import ctypes as C
+import dataclasses
 import math
 from dataclasses import dataclass, field
-from pathlib import Path
-from typing import Dict, List, Optional, Tuple, Union
+from typing import Dict, Optional, Tuple, Union
 
 import torch
 from torch import Tensor
 
 from . import _lib
-from .text_encoder import VocabularyInfo, sinusoidal_position_table
+from ._engine import EngineModel
+from .text_encoder import VocabularyInfo, _FrontendInfo, sinusoidal_position_table
 
 TOPK = 16  # candidates per row returned by sb_decoder_step (kTopkCandidates)
 
@@ -62,69 +62,44 @@ def sonar_text_decoder_config(arch: str = "basic", **overrides) -> SonarTextDeco
             num_encoder_layers=6, num_decoder_layers=6, ffn_inner_dim=1024 * 4)
     else:
         raise ValueError(f"unknown sonar text decoder arch {arch!r}")
-    for k, v in overrides.items():
-        if not hasattr(cfg, k):
-            raise TypeError(f"unknown config field {k!r}")
-        setattr(cfg, k, v)
-    return cfg
+    return dataclasses.replace(cfg, **overrides)
 
 
-class _PosInfo:
-    def __init__(self, n: int) -> None:
-        self.max_seq_len = n
-
-
-class _FrontendInfo:
-    def __init__(self, n: int) -> None:
-        self.pos_encoder = _PosInfo(n)
-
-
-class B200TextDecoderModel(torch.nn.Module):
+class B200TextDecoderModel(EngineModel):
     """SONAR text decoder (24 pre-LN layers + final LN + tied projection) on sm_90a kernels."""
+
+    _abi = "decoder"
+    _default_config = staticmethod(sonar_text_decoder_config)
 
     def __init__(self, config: SonarTextDecoderConfig, state_dict: Dict[str, Tensor],
                  device: Union[str, torch.device] = "cuda") -> None:
-        super().__init__()
+        super().__init__(device)
         if config.activation_fn != "ReLU" or config.layernorm_embedding or config.learned_pos \
                 or config.no_token_positional_embeddings or not config.normalize_before:
             raise NotImplementedError("sonar_b200 text decoder supports the `basic`/`small` wiring only")
         if config.input_dim not in (None, config.model_dim):
             raise NotImplementedError("input_dim != model_dim is not supported by the CUDA decoder")
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise RuntimeError("B200TextDecoderModel needs a CUDA device (there is no CPU path)")
-        if dev.index is None:
-            dev = torch.device("cuda", torch.cuda.current_device())
-        self.device = dev
         self.config = config
         self.model_dim = config.model_dim
         self.target_vocab_info = config.vocab_info
         pad = config.vocab_info.pad_idx if config.vocab_info.pad_idx is not None else 1
         # SinusoidalPositionEncoder(max_seq_len, _legacy_pad_idx=pad) as built at factory.py:248-252
         self.max_target_seq_len = config.max_seq_len
-        self.decoder_frontend = _FrontendInfo(config.max_seq_len)  # read by TextToTextModelPipeline (text.py:102)
-        self._lib = _lib.load()
+        self.decoder_frontend = _FrontendInfo(config.max_seq_len, config.model_dim)
         sd, d, L = state_dict, config.model_dim, config.num_decoder_layers
-
-        def bf(t):
-            return t.detach().to(device=dev, dtype=torch.bfloat16).contiguous()
-
-        def f32(t):
-            return t.detach().to(device=dev, dtype=torch.float32).contiguous()
+        bf, f32 = self._bf16, self._f32
 
         embed = sd["decoder_frontend.embed.weight"]
         if "final_proj.weight" in sd and sd["final_proj.weight"].data_ptr() != embed.data_ptr() \
                 and not torch.equal(sd["final_proj.weight"], embed):
             raise ValueError("final_proj.weight must be tied to decoder_frontend.embed.weight (factory.py:306-307)")
-        self.register_buffer("embed", bf(embed), persistent=False)
-        self.register_buffer("pos_table", sinusoidal_position_table(config.max_seq_len, d, pad).to(dev), persistent=False)
-        self.register_buffer("final_ln_g", f32(sd["decoder.layer_norm.weight"]), persistent=False)
-        self.register_buffer("final_ln_b", f32(sd["decoder.layer_norm.bias"]), persistent=False)
-        self._layer_bufs: List[Dict[str, Tensor]] = []
+        top = {"embed": bf(embed), "pos_table": f32(sinusoidal_position_table(config.max_seq_len, d, pad)),
+               "final_ln_g": f32(sd["decoder.layer_norm.weight"]), "final_ln_b": f32(sd["decoder.layer_norm.bias"])}
+        layers = []
         for i in range(L):
             p = f"decoder.layers.{i}."
             a, c = p + "self_attn.", p + "encoder_decoder_attn."
-            bufs = {
+            layers.append({
                 "wqkv": bf(torch.cat([sd[a + "q_proj.weight"], sd[a + "k_proj.weight"], sd[a + "v_proj.weight"]], 0)),
                 "bqkv": f32(torch.cat([sd[a + "q_proj.bias"], sd[a + "k_proj.bias"], sd[a + "v_proj.bias"]], 0)),
                 "wo": bf(sd[a + "output_proj.weight"]), "bo": f32(sd[a + "output_proj.bias"]),
@@ -134,56 +109,22 @@ class B200TextDecoderModel(torch.nn.Module):
                 "w2": bf(sd[p + "ffn.output_proj.weight"]), "b2": f32(sd[p + "ffn.output_proj.bias"]),
                 "ln1_g": f32(sd[p + "self_attn_layer_norm.weight"]), "ln1_b": f32(sd[p + "self_attn_layer_norm.bias"]),
                 "ln3_g": f32(sd[p + "ffn_layer_norm.weight"]), "ln3_b": f32(sd[p + "ffn_layer_norm.bias"]),
-            }
-            for k, v in bufs.items():
-                self.register_buffer(f"l{i}_{k}", v, persistent=False)
-            self._layer_bufs.append(bufs)
+            })
         cfg_c = _lib.SbDecoderConfig(
             model_dim=d, num_layers=L, num_heads=config.num_decoder_attn_heads, ffn_inner_dim=config.ffn_inner_dim,
             input_dim=config.input_dim or d, vocab_size=config.vocab_info.size, pos_rows=config.max_seq_len,
             eos_idx=config.vocab_info.eos_idx, ln_eps=1e-5,
             embed_scale=1.0 if config.no_scale_embedding else math.sqrt(d))
-        layers_c = (_lib.SbDecoderLayerWeights * max(L, 1))()
-        for i, bufs in enumerate(self._layer_bufs):
-            for k, v in bufs.items():
-                setattr(layers_c[i], k, v.data_ptr())
-        w_c = _lib.SbDecoderWeights(embed=self.embed.data_ptr(), pos_table=self.pos_table.data_ptr(),
-                                    final_ln_g=self.final_ln_g.data_ptr(), final_ln_b=self.final_ln_b.data_ptr(),
-                                    layers=layers_c)
-        handle = C.c_void_p()
-        with torch.cuda.device(dev):
-            _lib.check(self._lib.sb_decoder_create(C.byref(cfg_c), C.byref(w_c), C.byref(handle)), "sb_decoder_create")
-        self._handle = handle
-        self._workspace: Optional[Tensor] = None
+        w_c = _lib.SbDecoderWeights(layers=self._layer_array(_lib.SbDecoderLayerWeights, layers),
+                                    **{k: v.data_ptr() for k, v in top.items()})
+        self._create(cfg_c, w_c)
         self._shape: Optional[Tuple[int, int, int]] = None
-
-    @classmethod
-    def from_checkpoint(cls, path: Union[str, Path], config: Optional[SonarTextDecoderConfig] = None,
-                        device: Union[str, torch.device] = "cuda") -> "B200TextDecoderModel":
-        ckpt = torch.load(str(path), map_location="cpu", weights_only=True)
-        sd = ckpt["model"] if "model" in ckpt else ckpt
-        return cls(config or sonar_text_decoder_config("basic"), sd, device)
-
-    @property
-    def dtype(self) -> torch.dtype:
-        return torch.bfloat16
-
-    def __del__(self) -> None:  # pragma: no cover
-        try:
-            if getattr(self, "_handle", None):
-                self._lib.sb_decoder_destroy(self._handle)
-                self._handle = None
-        except Exception:
-            pass
-
-    def _stream(self) -> int:
-        return torch.cuda.current_stream(self.device).cuda_stream
 
     @torch.inference_mode()
     def begin(self, embeddings: Tensor, beam: int, max_len: int) -> None:
         """Start decoding a batch of sentence embeddings [N, model_dim] with `beam` hypotheses each and at most
         `max_len` positions (prompt included)."""
-        emb = embeddings.to(device=self.device, dtype=torch.float32).contiguous()
+        emb = self._on_device(embeddings, torch.float32).contiguous()
         if emb.dim() == 3 and emb.shape[1] == 1:
             emb = emb[:, 0].contiguous()
         n = emb.shape[0]
@@ -191,16 +132,11 @@ class B200TextDecoderModel(torch.nn.Module):
             raise ValueError(f"expected embeddings of shape [N, {self.model_dim}]")
         if max_len > self.max_target_seq_len:
             raise ValueError(f"max_len {max_len} exceeds the decoder's max_seq_len {self.max_target_seq_len}")
-        need = C.c_size_t()
-        _lib.check(self._lib.sb_decoder_workspace_bytes(self._handle, n, beam, max_len, C.byref(need)),
-                   "sb_decoder_workspace_bytes")
-        if self._workspace is None or self._workspace.numel() < need.value:
-            self._workspace = None
-            self._workspace = torch.empty(need.value + 4096, dtype=torch.uint8, device=self.device)
+        ws = self._ensure_workspace(n, beam, max_len)
         self._shape = (n, beam, max_len)
         with torch.cuda.device(self.device):
-            rc = self._lib.sb_decoder_begin(self._handle, emb.data_ptr(), n, beam, max_len, self._workspace.data_ptr(),
-                                            self._workspace.numel(), self._stream())
+            rc = self._lib.sb_decoder_begin(self._handle, emb.data_ptr(), n, beam, max_len, ws.data_ptr(), ws.numel(),
+                                            self._stream())
         _lib.check(rc, "sb_decoder_begin")
 
     @torch.inference_mode()

@@ -16,10 +16,10 @@ only repacks weights (bf16, fused QKV) and owns device buffers.
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import math
 from dataclasses import dataclass, field
 from enum import Enum
-from pathlib import Path
 from typing import Dict, List, Optional, Union
 
 import numpy as np
@@ -27,6 +27,7 @@ import torch
 from torch import Tensor
 
 from . import _lib, ops
+from ._engine import EngineModel
 from .sequence import PaddingMask, SequenceBatch, SonarEncoderOutput
 
 
@@ -87,11 +88,7 @@ def sonar_text_encoder_config(arch: str = "basic", **overrides) -> SonarTextEnco
             num_encoder_layers=6, num_decoder_layers=6, ffn_inner_dim=1024 * 4)
     else:
         raise ValueError(f"unknown sonar text encoder arch {arch!r}")
-    for k, v in overrides.items():
-        if not hasattr(cfg, k):
-            raise TypeError(f"unknown config field {k!r}")
-        setattr(cfg, k, v)
-    return cfg
+    return dataclasses.replace(cfg, **overrides)
 
 
 def sinusoidal_position_table(num_pos: int, dim: int, legacy_pad_idx: int) -> Tensor:
@@ -112,7 +109,8 @@ class _PosEncoderInfo:
 
 
 class _FrontendInfo:
-    """Carries ``encoder_frontend.pos_encoder.max_seq_len`` (read at ``text.py:202``)."""
+    """Carries ``encoder_frontend.pos_encoder.max_seq_len`` / ``decoder_frontend.pos_encoder.max_seq_len`` (read at
+    ``text.py:202`` and ``text.py:102``)."""
 
     def __init__(self, max_seq_len: int, model_dim: int) -> None:
         self.pos_encoder = _PosEncoderInfo(max_seq_len)
@@ -135,8 +133,11 @@ def _check_supported(cfg: SonarTextEncoderConfig) -> None:
         raise NotImplementedError("sonar_b200 text encoder does not support: " + "; ".join(bad))
 
 
-class B200TextEncoderModel(torch.nn.Module):
+class B200TextEncoderModel(EngineModel):
     """SONAR text encoder (24-layer pre-LN Transformer + final LN + pooling) on sm_90a kernels."""
+
+    _abi = "encoder"
+    _default_config = staticmethod(sonar_text_encoder_config)
 
     def __init__(self, config: SonarTextEncoderConfig, state_dict: Dict[str, Tensor],
                  device: Union[str, torch.device] = "cuda", *, cta_group: int = 2,
@@ -144,44 +145,30 @@ class B200TextEncoderModel(torch.nn.Module):
         """``ln_fold=True``: the engine folds every encoder-layer LayerNorm into the GEMMs around it (see
         ``SbEncoderConfig.ln_fold`` in ``include/sonar_b200.h``); the default runs the separate LayerNorm kernels
         (``bench.py`` A/Bs the schedules in every run, ``ab_schedule_variants``)."""
-        super().__init__()
+        super().__init__(device)
         self.ln_fold = int(ln_fold)  # 0 = separate LayerNorm kernels, 1 = both folded, 2 = only the attention-block one
         _check_supported(config)
         self.config = config
         self.model_dim = config.model_dim
         self.pooling = getattr(Pooling, config.pooling.upper())
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise RuntimeError("B200TextEncoderModel needs a CUDA device (there is no CPU path)")
-        if dev.index is None:
-            dev = torch.device("cuda", torch.cuda.current_device())
-        self.device = dev
         pad_idx = config.vocab_info.pad_idx if config.vocab_info.pad_idx is not None else 1
         max_len = config.max_seq_len + (pad_idx + 1 if config._from_fairseq else 0)  # factory.py:53-59
         self.encoder_frontend = _FrontendInfo(max_len, config.model_dim)
-        self._lib = _lib.load()
 
         sd = state_dict
         d, L = config.model_dim, config.num_encoder_layers
-
-        def bf(t: Tensor) -> Tensor:
-            return t.detach().to(device=dev, dtype=torch.bfloat16).contiguous()
-
-        def f32(t: Tensor) -> Tensor:
-            return t.detach().to(device=dev, dtype=torch.float32).contiguous()
+        bf, f32 = self._bf16, self._f32
 
         embed = sd["encoder_frontend.embed.weight"]
         if embed.shape != (config.vocab_info.size, d):
             raise ValueError(f"embedding shape {tuple(embed.shape)} != ({config.vocab_info.size}, {d})")
-        self.register_buffer("embed", bf(embed), persistent=False)
-        self.register_buffer("pos_table", sinusoidal_position_table(max_len, d, pad_idx).to(dev), persistent=False)
-        self.register_buffer("final_ln_g", f32(sd["layer_norm.weight"]), persistent=False)
-        self.register_buffer("final_ln_b", f32(sd["layer_norm.bias"]), persistent=False)
+        top = {"embed": bf(embed), "pos_table": f32(sinusoidal_position_table(max_len, d, pad_idx)),
+               "final_ln_g": f32(sd["layer_norm.weight"]), "final_ln_b": f32(sd["layer_norm.bias"])}
         self._layer_bufs: List[Dict[str, Tensor]] = []
         for i in range(L):
             p = f"encoder.layers.{i}."
             a = p + "self_attn."
-            bufs = {
+            self._layer_bufs.append({
                 "wqkv": bf(torch.cat([sd[a + "q_proj.weight"], sd[a + "k_proj.weight"], sd[a + "v_proj.weight"]], 0)),
                 "bqkv": f32(torch.cat([sd[a + "q_proj.bias"], sd[a + "k_proj.bias"], sd[a + "v_proj.bias"]], 0)),
                 "wo": bf(sd[a + "output_proj.weight"]), "bo": f32(sd[a + "output_proj.bias"]),
@@ -189,71 +176,24 @@ class B200TextEncoderModel(torch.nn.Module):
                 "w2": bf(sd[p + "ffn.output_proj.weight"]), "b2": f32(sd[p + "ffn.output_proj.bias"]),
                 "ln1_g": f32(sd[p + "self_attn_layer_norm.weight"]), "ln1_b": f32(sd[p + "self_attn_layer_norm.bias"]),
                 "ln2_g": f32(sd[p + "ffn_layer_norm.weight"]), "ln2_b": f32(sd[p + "ffn_layer_norm.bias"]),
-            }
-            for k, v in bufs.items():
-                self.register_buffer(f"l{i}_{k}", v, persistent=False)
-            self._layer_bufs.append(bufs)
+            })
 
         cfg_c = _lib.SbEncoderConfig(
             model_dim=d, num_layers=L, num_heads=config.num_encoder_attn_heads, ffn_inner_dim=config.ffn_inner_dim,
             vocab_size=config.vocab_info.size, pos_rows=max_len, pooling=self.pooling.value, ln_eps=1e-5,
             embed_scale=1.0 if config.no_scale_embedding else math.sqrt(d), cta_group=cta_group, num_sms=0,
             ln_fold=int(ln_fold))
-        layers_c = (_lib.SbLayerWeights * max(L, 1))()
-        for i, bufs in enumerate(self._layer_bufs):
-            for k, v in bufs.items():
-                setattr(layers_c[i], k, v.data_ptr())
-        w_c = _lib.SbEncoderWeights(embed=self.embed.data_ptr(), pos_table=self.pos_table.data_ptr(),
-                                    final_ln_g=self.final_ln_g.data_ptr(), final_ln_b=self.final_ln_b.data_ptr(),
-                                    layers=layers_c)
-        handle = C.c_void_p()
-        with torch.cuda.device(dev):
-            _lib.check(self._lib.sb_encoder_create(C.byref(cfg_c), C.byref(w_c), C.byref(handle)), "sb_encoder_create")
-        self._handle = handle
-        self._workspace: Optional[Tensor] = None
+        w_c = _lib.SbEncoderWeights(layers=self._layer_array(_lib.SbLayerWeights, self._layer_bufs),
+                                    **{k: v.data_ptr() for k, v in top.items()})
+        self._create(cfg_c, w_c)
         self.return_encoded_seqs = False
-
-    # ------------------------------------------------------------------ construction helpers
-    @classmethod
-    def from_checkpoint(cls, path: Union[str, Path], config: Optional[SonarTextEncoderConfig] = None,
-                        device: Union[str, torch.device] = "cuda", **kw) -> "B200TextEncoderModel":
-        """Load a fairseq2-layout checkpoint ``{"model": state_dict}`` (SURVEY App. A.3)."""
-        ckpt = torch.load(str(path), map_location="cpu", weights_only=True)
-        sd = ckpt["model"] if "model" in ckpt else ckpt
-        return cls(config or sonar_text_encoder_config("basic"), sd, device, **kw)
-
-    # ------------------------------------------------------------------ nn.Module-ish surface
-    @property
-    def dtype(self) -> torch.dtype:
-        """Compute dtype of the engine (bf16 operands, fp32 accumulation and residual stream)."""
-        return torch.bfloat16
-
-    def __del__(self) -> None:  # pragma: no cover - best effort
-        try:
-            if getattr(self, "_handle", None):
-                self._lib.sb_encoder_destroy(self._handle)
-                self._handle = None
-        except Exception:
-            pass
-
-    def _ensure_workspace(self, batch: int, tokens: int) -> Tensor:
-        need = C.c_size_t()
-        _lib.check(self._lib.sb_encoder_workspace_bytes(self._handle, batch, tokens, C.byref(need)),
-                   "sb_encoder_workspace_bytes")
-        if self._workspace is None or self._workspace.numel() < need.value:
-            self._workspace = None  # release before growing
-            self._workspace = torch.empty(int(need.value * 1.1) + 4096, dtype=torch.uint8, device=self.device)
-        return self._workspace
 
     @torch.inference_mode()
     def forward(self, batch: SequenceBatch) -> SonarEncoderOutput:
         seqs = batch.seqs
         if seqs.dim() != 2:
             raise ValueError("expected token ids of shape [N, S]")
-        if not seqs.is_cuda:
-            seqs = seqs.to(self.device, non_blocking=True)
-        if seqs.dtype != torch.int64:
-            seqs = seqs.to(torch.int64)
+        seqs = self._on_device(seqs, torch.int64)
         if seqs.stride(1) != 1:
             seqs = seqs.contiguous()
         n, s = seqs.shape
@@ -265,15 +205,14 @@ class B200TextEncoderModel(torch.nn.Module):
         else:
             lens_c = None
             tokens = n * s
-        ws = self._ensure_workspace(n, max(tokens, 1))
+        ws = self._ensure_workspace(n, max(tokens, 1), headroom=1.1)  # predict() grows it batch by batch
         out = torch.empty((n, self.model_dim), dtype=torch.float32, device=self.device)
         enc = (torch.empty((n, s, self.model_dim), dtype=torch.float32, device=self.device)
                if self.return_encoded_seqs else None)
         with torch.cuda.device(self.device):
             rc = self._lib.sb_encoder_forward(
                 self._handle, seqs.data_ptr(), seqs.stride(0), lens_c, n, s, out.data_ptr(),
-                enc.data_ptr() if enc is not None else None, ws.data_ptr(), ws.numel(),
-                torch.cuda.current_stream(self.device).cuda_stream)
+                enc.data_ptr() if enc is not None else None, ws.data_ptr(), ws.numel(), self._stream())
         _lib.check(rc, "sb_encoder_forward")
         return SonarEncoderOutput(encoded_seqs=enc, sentence_embeddings=out, padding_mask=pm)
 
@@ -288,9 +227,8 @@ class B200TextEncoderModel(torch.nn.Module):
         """Raise ``ValueError`` if the last batch contained a token id outside the vocabulary."""
         if self._workspace is None:
             return
-        rc = self._lib.sb_encoder_check_inputs(self._handle, self._workspace.data_ptr(),
-                                               torch.cuda.current_stream(self.device).cuda_stream)
-        _lib.check(rc, "sb_encoder_check_inputs")
+        _lib.check(self._lib.sb_encoder_check_inputs(self._handle, self._workspace.data_ptr(), self._stream()),
+                   "sb_encoder_check_inputs")
 
     # ------------------------------------------------------------------ reference static API
     @staticmethod
@@ -299,8 +237,7 @@ class B200TextEncoderModel(torch.nn.Module):
         ``seqs`` is a padded CUDA tensor [N, S, D] with D a multiple of 128."""
         if pooling == Pooling.ATTENTION:
             raise NotImplementedError(pooling)
-        if not seqs.is_cuda:
-            raise RuntimeError("static_pooling runs on CUDA tensors only")
+        ops._need_cuda(seqs)
         n, s, d = seqs.shape
         lens = padding_mask.seq_lens_host if padding_mask is not None else [s] * n
         valid = (torch.arange(s)[None, :] < torch.tensor(lens)[:, None]).to(seqs.device)

@@ -9,23 +9,20 @@ y matrix on every rank (the single exchange step of the path, SURVEY §8e), each
 
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional, Tuple
 
 import torch
 from torch import Tensor
 
 from . import _lib
+from .ops import _need_cuda
 
 _MARGINS = {"absolute": 0, "ratio": 1, "distance": 2}
 
 
 def _need_cuda_f32(t: Tensor) -> Tensor:
-    if not t.is_cuda:
-        raise RuntimeError("sonar_b200.xsim runs on CUDA tensors only (no CPU fallback exists)")
-    if t.dtype != torch.float32:
-        t = t.float()
-    return t.contiguous()
+    _need_cuda(t)
+    return t.float().contiguous()
 
 
 def knn(x: Tensor, y: Tensor, k: int = 4) -> Tuple[Tensor, Tensor]:
@@ -35,9 +32,7 @@ def knn(x: Tensor, y: Tensor, k: int = 4) -> Tuple[Tensor, Tensor]:
     m = y.shape[0]
     assert y.shape[1] == d
     lib = _lib.load()
-    need = C.c_size_t()
-    _lib.check(lib.sb_xsim_workspace_bytes(n, m, d, C.byref(need)), "sb_xsim_workspace_bytes")
-    ws = torch.empty(need.value, dtype=torch.uint8, device=x.device)
+    ws = torch.empty(_lib.workspace_bytes(lib.sb_xsim_workspace_bytes, n, m, d), dtype=torch.uint8, device=x.device)
     val = torch.empty((n, k), dtype=torch.float64, device=x.device)
     idx = torch.empty((n, k), dtype=torch.int32, device=x.device)
     with torch.cuda.device(x.device):
@@ -60,9 +55,7 @@ def knn_bidir(x: Tensor, y: Tensor, k: int = 4, stats: Optional[dict] = None) ->
     m = y.shape[0]
     assert y.shape[1] == d
     lib = _lib.load()
-    need = C.c_size_t()
-    _lib.check(lib.sb_xsim_bidir_workspace_bytes(n, m, d, C.byref(need)), "sb_xsim_bidir_workspace_bytes")
-    ws = torch.empty(need.value, dtype=torch.uint8, device=x.device)
+    ws = torch.empty(_lib.workspace_bytes(lib.sb_xsim_bidir_workspace_bytes, n, m, d), dtype=torch.uint8, device=x.device)
     val_xy = torch.empty((n, k), dtype=torch.float64, device=x.device)
     idx_xy = torch.empty((n, k), dtype=torch.int32, device=x.device)
     val_yx = torch.empty((m, k), dtype=torch.float64, device=x.device)

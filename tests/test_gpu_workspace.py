@@ -1,5 +1,7 @@
-"""Every C-ABI entry point that carves the caller's workspace rejects one that is too small (SB_ERR_INVALID, a message that
-names the entry point) instead of writing past its end.  Engines are the small configurations of the other GPU tests."""
+"""The engines' host side: every C-ABI entry point that carves the caller's workspace rejects one that is too small
+(SB_ERR_INVALID, a message that names the entry point) instead of writing past its end, and the Python wrappers keep the
+weights the engines point into out of reach of ``nn.Module`` conversions.  Engines are the small configurations of the
+other GPU tests."""
 
 import ctypes as C
 
@@ -75,3 +77,41 @@ def test_too_small_workspace_is_rejected(engines, cuda_device):
         assert rc == _lib.SB_ERR_INVALID, (name, rc, msg)
         assert msg.startswith(f"{name}: workspace too small"), (name, msg)
     torch.cuda.synchronize(dev)
+
+
+def test_module_conversions_leave_the_engines_alone(engines, cuda_device):
+    """No engine weight is a buffer or a parameter, so ``.half()``, ``.to(dtype)`` and ``.to(device)`` have nothing to
+    replace (or free while the engine still reads it): the outputs afterwards are bitwise those from before.  The inputs
+    start on the CPU, so each wrapper also moves them to its device."""
+    from sonar_b200 import PaddingMask, SequenceBatch
+
+    encoder, decoder, speech = engines
+    g = torch.Generator().manual_seed(7)
+    ids = torch.randint(4, VOCAB, (3, 16), generator=g)
+    fb = torch.randn((2, 40, 80), generator=g)
+    emb = torch.randn((3, 1024), generator=g) * 0.25
+    beam, max_len = 2, 8
+    tokens = torch.full((3 * beam,), 2, dtype=torch.int64, device=cuda_device)
+    table = torch.arange(3 * beam, dtype=torch.int32, device=cuda_device)[:, None].expand(3 * beam, max_len).contiguous()
+
+    def decode():
+        decoder.begin(emb, beam, max_len)
+        return decoder.step(tokens, table, 0)
+
+    runs = [
+        (encoder, lambda: [encoder(SequenceBatch(ids, PaddingMask(torch.tensor([16, 9, 1]), 16, [16, 9, 1])))
+                           .sentence_embeddings]),
+        (decoder, decode),
+        (speech, lambda: [speech(SequenceBatch(fb, PaddingMask(torch.tensor([40, 23]), 40, [40, 23])))
+                          .sentence_embeddings]),
+    ]
+    for model, run in runs:
+        name = type(model).__name__
+        assert list(model.buffers()) == [] and list(model.parameters()) == [], name
+        before = [t.clone() for t in run()]
+        model.half()
+        model.to(torch.bfloat16)
+        model.to(cuda_device)
+        after = run()
+        torch.cuda.synchronize(cuda_device)
+        assert all(torch.equal(a, b) for a, b in zip(before, after)), name

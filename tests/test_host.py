@@ -139,10 +139,40 @@ def test_no_cpu_fallback_in_product():
             if f.endswith(".py"):
                 src = open(os.path.join(dirpath, f)).read()
                 assert "import oracle" not in src and "from oracle" not in src, f
-    from sonar_b200.text_encoder import B200TextEncoderModel, sonar_text_encoder_config
+    from sonar_b200 import (B200SpeechEncoderModel, B200TextDecoderModel, B200TextEncoderModel,
+                            sonar_speech_encoder_config, sonar_text_decoder_config, sonar_text_encoder_config)
 
-    with pytest.raises(RuntimeError, match="CUDA"):
-        B200TextEncoderModel(sonar_text_encoder_config("basic"), {}, device="cpu")
+    # the device is checked before the (empty) state dict is read
+    for cls, config in ((B200TextEncoderModel, sonar_text_encoder_config()),
+                        (B200TextDecoderModel, sonar_text_decoder_config()),
+                        (B200SpeechEncoderModel, sonar_speech_encoder_config())):
+        with pytest.raises(RuntimeError, match="CUDA"):
+            cls(config, {}, device="cpu")
+
+
+def test_annotations_resolve():
+    """Every annotation in the package names something importable (``from __future__ import annotations`` defers them,
+    so an unimported name only shows when a caller such as ``dataclasses`` tooling asks for ``get_type_hints``)."""
+    import importlib
+    import inspect
+    import pkgutil
+    import typing
+
+    import sonar_b200
+
+    for info in pkgutil.walk_packages(sonar_b200.__path__, "sonar_b200."):
+        mod = importlib.import_module(info.name)
+        for obj in vars(mod).values():
+            if getattr(obj, "__module__", None) != mod.__name__:
+                continue
+            if inspect.isclass(obj):
+                targets = [obj] + [f for f in vars(obj).values() if inspect.isfunction(f)]
+            elif inspect.isfunction(obj):
+                targets = [obj]
+            else:
+                continue
+            for t in targets:
+                typing.get_type_hints(t)  # NameError on an annotation that names nothing
 
 
 def test_tsv_manifest_reader(tmp_path):
