@@ -22,6 +22,8 @@
  *          PaddingMask(seq_lens).
  *   sb_pool
  *       <- SonarTextTransformerEncoderModel.static_pooling (model.py:86-128).
+ *   SB_POOL_ATTENTION / sb_pool_latent_attention
+ *       <- the attention pooler of SonarTextEncoderFactory.create_attention_pooler (factory.py:155-226).
  *   weight layout
  *       <- fairseq2 state-dict names mapped in sonar/models/sonar_text/handler.py:71-92
  *          (nn.Linear [out,in] row-major).
@@ -46,6 +48,7 @@ extern "C" {
 #define SB_POOL_MAX 1
 #define SB_POOL_MEAN 2
 #define SB_POOL_LAST 3
+#define SB_POOL_ATTENTION 4 /* trainable attention pooler (SonarTextEncoderFactory.create_attention_pooler, factory.py:155-226) */
 
 /* GEMM epilogues */
 #define SB_EPI_BIAS 0
@@ -76,6 +79,14 @@ typedef struct SbEncoderConfig {
                           * 2 = fold only the attention-block LayerNorm (FFN2 emits, QKV applies); the FFN-block LayerNorm
                           *     stays a kernel (the out-projection is HBM-bound, its epilogue has no slack for the extra work);
                           * 0 = separate LayerNorm kernels */
+  /* Attention pooling (pooling = SB_POOL_ATTENTION; the four fields are ignored otherwise, except embedding_dim):
+   * one BOS query through `pooler_layers` POST-LN decoder layers cross-attending the final-LayerNormed token states,
+   * then projection_out (with bias) -> [batch, embedding_dim] (factory.py:155-226). */
+  int32_t embedding_dim;        /* width E of `out`: multiple of 256, <= 1024, = 64 * pooler_heads; without attention
+                                 * pooling it must be 0 or model_dim (0 = model_dim) */
+  int32_t pooler_layers;        /* num_decoder_layers (24 for `basic`), >= 1 */
+  int32_t pooler_heads;         /* num_decoder_attn_heads (head dim 64, <= 16 heads) */
+  int32_t pooler_ffn_inner_dim; /* decoder_ffn_inner_dim, or ffn_inner_dim when that is None (multiple of 256) */
 } SbEncoderConfig;
 
 /* All pointers are DEVICE pointers and stay owned by the caller (must outlive the handle).
@@ -101,13 +112,22 @@ typedef struct SbEncoderWeights {
   const float* final_ln_g;     /* layer_norm.weight */
   const float* final_ln_b;     /* layer_norm.bias */
   const SbLayerWeights* layers; /* HOST array of num_layers entries (copied at create) */
+  /* attention pooling only (NULL otherwise); E = embedding_dim.  pooler[i] uses SbPoolerLayerWeights (declared with the
+   * speech encoder below) with every matrix [E, E] except ca_wkv = bf16 [2E, D] (k_proj | v_proj of
+   * encoder_decoder_attn, whose inputs are the D-wide token states), ca_bkv [2E], w1 [F_pool, E], w2 [E, F_pool] */
+  const float* pooler_q0;       /* fp32 [E] = pooler.decoder_frontend.embed.weight[0] * sqrt(E) + pos[0] */
+  const void* proj_w;           /* pooler.projection_out.weight bf16 [E, E] */
+  const float* proj_b;          /* pooler.projection_out.bias [E] */
+  const struct SbPoolerLayerWeights* pooler; /* HOST array of pooler_layers entries (copied at create) */
 } SbEncoderWeights;
 
 const char* sb_last_error(void);
 int sb_version(void);
 
 /* Allocates the handle's own device memory (a 256-byte input-check flag; with cfg->ln_fold the folded copies of the QKV and
- * FFN inner-projection weights, ~22 MB per layer) and synchronises the device once.  sb_encoder_forward never allocates. */
+ * FFN inner-projection weights, ~22 MB per layer; with attention pooling the absorbed cross-attention weights of every pooler
+ * layer, 2 * Hd * D * E * 2 + (Hd * D + E) * 4 bytes = 64 MB per layer at D = E = 1024, 16 heads) and synchronises the
+ * device once.  sb_encoder_forward never allocates. */
 int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbEncoder** out);
 void sb_encoder_destroy(SbEncoder* enc);
 
@@ -118,7 +138,7 @@ int sb_encoder_workspace_bytes(const SbEncoder* enc, int32_t max_batch, int64_t 
 /* One pass of the hot path.
  *   ids            DEVICE int64 [batch, ids_row_stride >= seq_len], right-padded (any pad value)
  *   seq_lens_host  HOST int32 [batch] true lengths (1..seq_len); NULL = every row is full (no padding_mask)
- *   out            DEVICE fp32 [batch, model_dim] sentence embeddings
+ *   out            DEVICE fp32 [batch, embedding_dim] sentence embeddings
  *   encoded        DEVICE fp32 [batch, seq_len, model_dim] or NULL (final-LayerNormed states, padded rows zeroed)
  * Asynchronous on `stream` (does not synchronise). */
 int sb_encoder_forward(SbEncoder* enc, const int64_t* ids, int64_t ids_row_stride, const int32_t* seq_lens_host,
@@ -128,7 +148,7 @@ int sb_encoder_forward(SbEncoder* enc, const int64_t* ids, int64_t ids_row_strid
 /* Same, but `ids_host` / `out_host` are HOST buffers (pinned for full speed); performs the
  * H2D copy of the ids, the forward and the D2H copy of the embeddings on `stream`, then
  * synchronises the stream.  `ids_staging` is DEVICE int64 [batch*seq_len], `out_staging`
- * DEVICE fp32 [batch*model_dim] (caller-owned). */
+ * DEVICE fp32 [batch*embedding_dim] (caller-owned). */
 int sb_encoder_forward_host(SbEncoder* enc, const int64_t* ids_host, const int32_t* seq_lens_host, int32_t batch,
                             int32_t seq_len, float* out_host, int64_t* ids_staging, float* out_staging,
                             void* workspace, size_t workspace_bytes, void* stream);
@@ -195,6 +215,13 @@ int sb_embed(const int64_t* ids, int64_t ids_row_stride, const int32_t* cu_seqle
 int sb_pool(const float* x, const int32_t* cu_seqlens, int32_t B, int32_t D, const float* gamma, const float* beta,
             float eps, int32_t apply_ln, int32_t pool_mode, float* out, float* encoded_padded, int32_t S_padded,
             void* stream);
+
+/* The attention pooler's cross-attention on the absorbed form (see SbEncoderWeights.pooler): qt DEVICE bf16 [B, Hd, D]
+ * (Hd <= 16 absorbed queries per sentence), mem DEVICE bf16 [total_tokens, D] packed rows (row cu_seqlens[b] + t),
+ * cu_seqlens DEVICE int32 [B+1]; u DEVICE bf16 [B, Hd, D] = softmax_t(qt[b,h,:] . mem[t,:] / 8) . mem over sentence b's
+ * rows (zeros for an empty sentence).  D in {256, 512, 768, 1024}. */
+int sb_pool_latent_attention(const void* qt, const void* mem, const int32_t* cu_seqlens, int32_t B, int32_t Hd, int32_t D,
+                             void* u, void* stream);
 
 /* ---- embedding -> text decoder, one incremental step at a time (BASELINE.json config 4) ----
  * Replaces ConditionalTransformerDecoderModel.decode + project (sonar/nn/conditional_decoder_model.py:60-94,

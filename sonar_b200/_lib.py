@@ -13,7 +13,7 @@ from typing import Optional
 _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libsonar_b200.so"
 _lib: Optional[C.CDLL] = None
 
-SB_POOL_MAX, SB_POOL_MEAN, SB_POOL_LAST = 1, 2, 3
+SB_POOL_MAX, SB_POOL_MEAN, SB_POOL_LAST, SB_POOL_ATTENTION = 1, 2, 3, 4
 SB_EPI_BIAS, SB_EPI_BIAS_RELU, SB_EPI_BIAS_RESIDUAL = 0, 1, 2
 SB_ERR_INVALID, SB_ERR_CUDA, SB_ERR_DRIVER, SB_ERR_INPUT = -1, -2, -3, -4
 
@@ -24,6 +24,8 @@ class SbEncoderConfig(C.Structure):
         ("ffn_inner_dim", C.c_int32), ("vocab_size", C.c_int64), ("pos_rows", C.c_int32),
         ("pooling", C.c_int32), ("ln_eps", C.c_float), ("embed_scale", C.c_float),
         ("cta_group", C.c_int32), ("num_sms", C.c_int32), ("ln_fold", C.c_int32),
+        ("embedding_dim", C.c_int32), ("pooler_layers", C.c_int32), ("pooler_heads", C.c_int32),
+        ("pooler_ffn_inner_dim", C.c_int32),
     ]
 
 
@@ -32,9 +34,17 @@ class SbLayerWeights(C.Structure):
         "wqkv", "bqkv", "wo", "bo", "w1", "b1", "w2", "b2", "ln1_g", "ln1_b", "ln2_g", "ln2_b")]
 
 
+class SbPoolerLayerWeights(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in (
+        "sa_wv", "sa_bv", "sa_wo", "sa_bo", "sa_ln_g", "sa_ln_b", "ca_wq", "ca_bq", "ca_wkv", "ca_bkv", "ca_wo", "ca_bo",
+        "ca_ln_g", "ca_ln_b", "w1", "b1", "w2", "b2", "ffn_ln_g", "ffn_ln_b")]
+
+
 class SbEncoderWeights(C.Structure):
     _fields_ = [("embed", C.c_void_p), ("pos_table", C.c_void_p), ("final_ln_g", C.c_void_p),
-                ("final_ln_b", C.c_void_p), ("layers", C.POINTER(SbLayerWeights))]
+                ("final_ln_b", C.c_void_p), ("layers", C.POINTER(SbLayerWeights)),
+                ("pooler_q0", C.c_void_p), ("proj_w", C.c_void_p), ("proj_b", C.c_void_p),
+                ("pooler", C.POINTER(SbPoolerLayerWeights))]
 
 
 class SbDecoderConfig(C.Structure):
@@ -69,12 +79,6 @@ class SbConformerLayerWeights(C.Structure):
         "ffn2_ln_g", "ffn2_ln_b", "ffn2_w1", "ffn2_b1", "ffn2_w2", "ffn2_b2", "ln_g", "ln_b")]
 
 
-class SbPoolerLayerWeights(C.Structure):
-    _fields_ = [(n, C.c_void_p) for n in (
-        "sa_wv", "sa_bv", "sa_wo", "sa_bo", "sa_ln_g", "sa_ln_b", "ca_wq", "ca_bq", "ca_wkv", "ca_bkv", "ca_wo", "ca_bo",
-        "ca_ln_g", "ca_ln_b", "w1", "b1", "w2", "b2", "ffn_ln_g", "ffn_ln_b")]
-
-
 class SbSpeechWeights(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("front_ln_g", "front_ln_b", "front_w", "front_b", "final_ln_g", "final_ln_b",
                                           "pooler_q0", "proj_w", "zeros")] + \
@@ -106,6 +110,8 @@ _SIGNATURES = {
                            C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_float,
                           C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "sb_pool_latent_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                           C.c_void_p, C.c_void_p]),
     "sb_decoder_create": (C.c_int, [C.POINTER(SbDecoderConfig), C.POINTER(SbDecoderWeights), C.POINTER(C.c_void_p)]),
     "sb_decoder_destroy": (None, [C.c_void_p]),
     "sb_decoder_workspace_bytes": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]),

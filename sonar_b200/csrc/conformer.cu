@@ -542,15 +542,6 @@ pool_attention_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* 
   *reinterpret_cast<uint32_t*>(out + (long long)b * D + h * 64 + lane * 2) = pack_bf16x2(a0 * inv, a1 * inv);
 }
 
-__global__ void broadcast_rows_kernel(const float* __restrict__ v, float* __restrict__ x, __nv_bfloat16* __restrict__ xb,
-                                      int B, int D) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)B * D) return;
-  const float f = v[i % D];
-  x[i] = f;
-  xb[i] = __float2bfloat16_rn(f);
-}
-
 }  // namespace
 }  // namespace sb
 
@@ -760,8 +751,7 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
   if ((rc = layernorm_dual(w.x, e->w.final_ln_g, e->w.final_ln_b, eps, w.x, w.e, T, D, stream))) return rc;
   if (encoded_packed) SB_CUDA_CHECK(cudaMemcpyAsync(encoded_packed, w.x, sizeof(float) * (size_t)T * D, cudaMemcpyDeviceToDevice, stream));
   // ---- attention pooler ----
-  broadcast_rows_kernel<<<(unsigned)(((long long)B * D + 255) / 256), 256, 0, stream>>>(e->w.pooler_q0, w.px, w.ph, B, D);
-  SB_CUDA_CHECK(cudaGetLastError());
+  if ((rc = broadcast_rows(e->w.pooler_q0, w.px, w.ph, B, D, stream))) return rc;
   for (int li = 0; li < e->cfg.pooler_layers; ++li) {
     const SbPoolerLayerWeights& P = e->pool[li];
     // self-attention over the single query token == Wo(Wv x + bv) + bo

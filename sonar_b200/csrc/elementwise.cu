@@ -176,6 +176,22 @@ layernorm_dual_kernel(const float* x, const float* __restrict__ gamma, const flo
   }
 }
 
+// x[b, :] = v, xb[b, :] = bf16(v) for every b < B: the single decoder position both attention poolers start from
+__global__ void broadcast_rows_kernel(const float* __restrict__ v, float* __restrict__ x, __nv_bfloat16* __restrict__ xb,
+                                      int B, int D) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)B * D) return;
+  const float f = v[i % D];
+  x[i] = f;
+  xb[i] = __float2bfloat16_rn(f);
+}
+
+int broadcast_rows(const float* v, float* x, __nv_bfloat16* xb, int B, int D, cudaStream_t stream) {
+  broadcast_rows_kernel<<<(unsigned)(((long long)B * D + 255) / 256), 256, 0, stream>>>(v, x, xb, B, D);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
 int layernorm_bf16(const float* x, const float* gamma, const float* beta, float eps, __nv_bfloat16* y, long long T,
                    int D, cudaStream_t stream) {
   if (T <= 0) return 0;

@@ -223,6 +223,21 @@ int attention_relpos_tc(const __nv_bfloat16* qkv, const __nv_bfloat16* p, const 
                         const int32_t* cu_seqlens, int B, int H, long long total_tokens, int Npad, int S_center,
                         __nv_bfloat16* qu, __nv_bfloat16* qv, __nv_bfloat16* out, int num_sms, cudaStream_t stream);
 
+// x [B, D] fp32 and xb [B, D] bf16 = B copies of the fp32 row v [D] (the attention poolers' single query position)
+int broadcast_rows(const float* v, float* x, __nv_bfloat16* xb, int B, int D, cudaStream_t stream);
+
+// Text attention pooler (latent_attention.cu).  u [B, Hd, D] bf16 = softmax_t(qt[b, h, :] . mem[t, :] / 8) . mem over the
+// rows t of sentence b in the packed memory mem [T, D] bf16; qt [B, Hd, D] bf16; Hd <= 16; D in {256, 512, 768, 1024};
+// an empty sentence gives zeros.
+int pool_latent_attention(const __nv_bfloat16* qt, const __nv_bfloat16* mem, const int32_t* cu_seqlens, int B, int Hd, int D,
+                          __nv_bfloat16* u, cudaStream_t stream);
+// Absorbs the cross-attention projections of one pooler layer (kv width D, pooler width E = 64 Hd) so that the layer runs
+// on pool_latent_attention: wqk [Hd*D, E] / bqk [Hd*D] map the pooler state to the absorbed queries
+// (qt_h = W_k,h^T (W_q,h x + b_q,h)); wvo [E, Hd*D] / bvo [E] map u to the attention output (W_o blockdiag(W_v,h) u +
+// W_o b_v + b_o).  The key bias drops out (softmax is shift-invariant).
+int absorb_pooler_weights(const SbPoolerLayerWeights& P, int D, int E, __nv_bfloat16* wqk, float* bqk, __nv_bfloat16* wvo,
+                          float* bvo, cudaStream_t stream);
+
 // optional final LayerNorm + pooling over packed sequences -> out [B, D] fp32;
 // optionally also scatters the (normalised) rows to a padded [B, S, D] fp32 tensor.
 int ln_pool(const float* x, const int32_t* cu_seqlens, int B, int D, const float* gamma, const float* beta,

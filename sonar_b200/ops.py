@@ -175,3 +175,19 @@ def pool_packed(x: Tensor, cu_seqlens: Tensor, pooling: str, *, gamma: Optional[
                              _ptr(enc), encoded_seq_len, _stream())
     _lib.check(rc, "sb_pool")
     return (out, enc) if enc is not None else out
+
+
+def pool_latent_attention(qt: Tensor, mem: Tensor, cu_seqlens: Tensor) -> Tensor:
+    """The attention pooler's cross-attention on the absorbed form: qt bf16 [B, Hd, D] (Hd <= 16 queries per sentence),
+    mem bf16 [T, D] packed rows, cu_seqlens int32 [B+1] -> u bf16 [B, Hd, D] with
+    u[b, h] = softmax_t(qt[b, h] . mem[t] / 8) . mem over the rows of sentence b (zeros for an empty sentence)."""
+    _need_cuda(qt, mem, cu_seqlens)
+    assert qt.dtype == torch.bfloat16 and mem.dtype == torch.bfloat16 and cu_seqlens.dtype == torch.int32
+    assert qt.is_contiguous() and mem.is_contiguous() and qt.dim() == 3 and mem.dim() == 2
+    b, hd, d = qt.shape
+    assert mem.shape[1] == d and cu_seqlens.numel() == b + 1
+    u = torch.empty_like(qt)
+    rc = _lib.load().sb_pool_latent_attention(qt.data_ptr(), mem.data_ptr(), cu_seqlens.data_ptr(), b, hd, d,
+                                              u.data_ptr(), _stream())
+    _lib.check(rc, "sb_pool_latent_attention")
+    return u

@@ -117,24 +117,51 @@ class _FrontendInfo:
         self.model_dim = model_dim
 
 
+def _embedding_dim(cfg: SonarTextEncoderConfig) -> int:
+    """Width of the sentence embeddings (``SonarTextEncoderFactory.embedding_dim``, ``factory.py:66-69``)."""
+    return cfg.embedding_dim or cfg.model_dim
+
+
+def _pooler_ffn_inner_dim(cfg: SonarTextEncoderConfig) -> int:
+    """Inner width of the attention pooler's FFNs (``create_ffn(inner_dim=decoder_ffn_inner_dim)``, ``factory.py:143-148``)."""
+    return cfg.decoder_ffn_inner_dim or cfg.ffn_inner_dim
+
+
 def _check_supported(cfg: SonarTextEncoderConfig) -> None:
     bad = []
-    if cfg.pooling.lower() not in ("mean", "max", "last"):
-        bad.append(f"pooling={cfg.pooling!r} (attention pooling is not on the H100 hot path yet)")
+    pooling = cfg.pooling.lower()
+    if pooling not in ("mean", "max", "last", "attention"):
+        bad.append(f"pooling={cfg.pooling!r}")
     if cfg.activation_fn != "ReLU":
         bad.append(f"activation_fn={cfg.activation_fn!r}")
     if cfg.layernorm_embedding or cfg.no_token_positional_embeddings or cfg.learned_pos:
         bad.append("layernorm_embedding / no_token_positional_embeddings / learned_pos")
-    if cfg.embedding_dim not in (None, cfg.model_dim):
-        bad.append("embedding_dim != model_dim")
     if cfg.model_dim != 64 * cfg.num_encoder_attn_heads:
         bad.append("head_dim != 64")
+    e = _embedding_dim(cfg)
+    if pooling != "attention":
+        if e != cfg.model_dim:
+            bad.append("embedding_dim != model_dim without attention pooling")
+    else:
+        if e % 256 != 0 or e > 1024 or e != 64 * cfg.num_decoder_attn_heads:
+            bad.append(f"attention pooling with embedding_dim={e}, num_decoder_attn_heads={cfg.num_decoder_attn_heads} "
+                       "(needs a multiple of 256, <= 1024, head_dim 64)")
+        if _pooler_ffn_inner_dim(cfg) % 256 != 0:
+            bad.append(f"attention pooling with a pooler FFN width of {_pooler_ffn_inner_dim(cfg)} (needs a multiple of 256)")
+        if cfg.num_decoder_layers < 1:
+            bad.append("attention pooling with num_decoder_layers < 1")
+        if cfg.normalize_before:
+            bad.append("attention pooling with normalize_before=True (a PRE-LN pooler)")
     if bad:
         raise NotImplementedError("sonar_b200 text encoder does not support: " + "; ".join(bad))
 
 
 class B200TextEncoderModel(EngineModel):
-    """SONAR text encoder (24-layer pre-LN Transformer + final LN + pooling) on sm_90a kernels."""
+    """SONAR text encoder (24-layer pre-LN Transformer + final LN + pooling) on sm_90a kernels.
+
+    ``pooling="attention"`` runs the reference's trainable pooler (``factory.py:155-226``): one BOS query through
+    ``num_decoder_layers`` POST-LN decoder layers cross-attending the final-LayerNormed token states, then
+    ``projection_out``; the sentence embeddings are ``embedding_dim`` wide."""
 
     _abi = "encoder"
     _default_config = staticmethod(sonar_text_encoder_config)
@@ -150,6 +177,7 @@ class B200TextEncoderModel(EngineModel):
         _check_supported(config)
         self.config = config
         self.model_dim = config.model_dim
+        self.embedding_dim = _embedding_dim(config)
         self.pooling = getattr(Pooling, config.pooling.upper())
         pad_idx = config.vocab_info.pad_idx if config.vocab_info.pad_idx is not None else 1
         max_len = config.max_seq_len + (pad_idx + 1 if config._from_fairseq else 0)  # factory.py:53-59
@@ -178,15 +206,53 @@ class B200TextEncoderModel(EngineModel):
                 "ln2_g": f32(sd[p + "ffn_layer_norm.weight"]), "ln2_b": f32(sd[p + "ffn_layer_norm.bias"]),
             })
 
+        attn = self.pooling == Pooling.ATTENTION
+        pooler_layers = self._pooler_weights(sd, top) if attn else []
         cfg_c = _lib.SbEncoderConfig(
             model_dim=d, num_layers=L, num_heads=config.num_encoder_attn_heads, ffn_inner_dim=config.ffn_inner_dim,
             vocab_size=config.vocab_info.size, pos_rows=max_len, pooling=self.pooling.value, ln_eps=1e-5,
             embed_scale=1.0 if config.no_scale_embedding else math.sqrt(d), cta_group=cta_group, num_sms=0,
-            ln_fold=int(ln_fold))
+            ln_fold=int(ln_fold), embedding_dim=self.embedding_dim,
+            pooler_layers=config.num_decoder_layers if attn else 0,
+            pooler_heads=config.num_decoder_attn_heads if attn else 0,
+            pooler_ffn_inner_dim=_pooler_ffn_inner_dim(config) if attn else 0)
         w_c = _lib.SbEncoderWeights(layers=self._layer_array(_lib.SbLayerWeights, self._layer_bufs),
                                     **{k: v.data_ptr() for k, v in top.items()})
+        if attn:
+            w_c.pooler = self._layer_array(_lib.SbPoolerLayerWeights, pooler_layers)
         self._create(cfg_c, w_c)
         self.return_encoded_seqs = False
+
+    def _pooler_weights(self, sd: Dict[str, Tensor], top: Dict[str, Tensor]) -> List[Dict[str, Tensor]]:
+        """The attention pooler's tensors in the engine's layout (``SbEncoderWeights.pooler_q0 / proj_w / proj_b``
+        added to ``top``; one ``SbPoolerLayerWeights`` dict per decoder layer)."""
+        e = self.embedding_dim
+        bf, f32 = self._bf16, self._f32
+        # the single decoder input: TransformerEmbeddingFrontend of token bos_idx = 0 = embed[0] * sqrt(E) + the
+        # sinusoid of position 0, [sin 0 ... | cos 0 ...] = [0 ... | 1 ...]  [fs2]
+        pos0 = torch.cat([torch.zeros(e // 2), torch.ones(e - e // 2)])
+        top["pooler_q0"] = f32(sd["pooler.decoder_frontend.embed.weight"][0].float() * math.sqrt(e) + pos0)
+        top["proj_w"] = bf(sd["pooler.projection_out.weight"])
+        top["proj_b"] = f32(sd["pooler.projection_out.bias"])
+        layers = []
+        for i in range(self.config.num_decoder_layers):
+            p = f"pooler.decoder.layers.{i}."
+            sa, ca = p + "self_attn.", p + "encoder_decoder_attn."
+            layers.append({
+                "sa_wv": bf(sd[sa + "v_proj.weight"]), "sa_bv": f32(sd[sa + "v_proj.bias"]),
+                "sa_wo": bf(sd[sa + "output_proj.weight"]), "sa_bo": f32(sd[sa + "output_proj.bias"]),
+                "sa_ln_g": f32(sd[p + "self_attn_layer_norm.weight"]), "sa_ln_b": f32(sd[p + "self_attn_layer_norm.bias"]),
+                "ca_wq": bf(sd[ca + "q_proj.weight"]), "ca_bq": f32(sd[ca + "q_proj.bias"]),
+                "ca_wkv": bf(torch.cat([sd[ca + "k_proj.weight"], sd[ca + "v_proj.weight"]], 0)),
+                "ca_bkv": f32(torch.cat([sd[ca + "k_proj.bias"], sd[ca + "v_proj.bias"]], 0)),
+                "ca_wo": bf(sd[ca + "output_proj.weight"]), "ca_bo": f32(sd[ca + "output_proj.bias"]),
+                "ca_ln_g": f32(sd[p + "encoder_decoder_attn_layer_norm.weight"]),
+                "ca_ln_b": f32(sd[p + "encoder_decoder_attn_layer_norm.bias"]),
+                "w1": bf(sd[p + "ffn.inner_proj.weight"]), "b1": f32(sd[p + "ffn.inner_proj.bias"]),
+                "w2": bf(sd[p + "ffn.output_proj.weight"]), "b2": f32(sd[p + "ffn.output_proj.bias"]),
+                "ffn_ln_g": f32(sd[p + "ffn_layer_norm.weight"]), "ffn_ln_b": f32(sd[p + "ffn_layer_norm.bias"]),
+            })
+        return layers
 
     @torch.inference_mode()
     def forward(self, batch: SequenceBatch) -> SonarEncoderOutput:
@@ -206,7 +272,7 @@ class B200TextEncoderModel(EngineModel):
             lens_c = None
             tokens = n * s
         ws = self._ensure_workspace(n, max(tokens, 1), headroom=1.1)  # predict() grows it batch by batch
-        out = torch.empty((n, self.model_dim), dtype=torch.float32, device=self.device)
+        out = torch.empty((n, self.embedding_dim), dtype=torch.float32, device=self.device)
         enc = (torch.empty((n, s, self.model_dim), dtype=torch.float32, device=self.device)
                if self.return_encoded_seqs else None)
         with torch.cuda.device(self.device):
