@@ -369,6 +369,10 @@ typedef struct SbSpeechWeights {
   const SbPoolerLayerWeights* pooler;
 } SbSpeechWeights;
 
+/* Allocates the handle's own device memory, the absorbed cross-attention weights of every pooler layer (as for
+ * sb_encoder_create with E = D and Hd = num_heads: 2 * Hd * D * D * 2 + (Hd * D + D) * 4 bytes = 64 MB per layer at
+ * D = 1024, so 192 MB for `english` and 384 MB for `non_english`), and synchronises the device once.
+ * sb_speech_encoder_forward never allocates. */
 int sb_speech_encoder_create(const SbSpeechConfig* cfg, const SbSpeechWeights* w, SbSpeechEncoder** out);
 void sb_speech_encoder_destroy(SbSpeechEncoder* enc);
 int sb_speech_encoder_workspace_bytes(const SbSpeechEncoder* enc, int32_t batch, int64_t total_positions,

@@ -3,8 +3,9 @@
 from __future__ import annotations
 
 import ctypes as C
+import math
 from pathlib import Path
-from typing import Any, Callable, Dict, List, Optional, Union
+from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 
 import torch
 from torch import Tensor
@@ -74,6 +75,39 @@ class EngineModel(torch.nn.Module):
             for name, _ in struct._fields_:
                 setattr(arr[i], name, tensors[name].data_ptr())
         return arr
+
+    def _pooler_weights(self, sd: Dict[str, Tensor], prefix: str, bos_idx: int,
+                        width: int) -> Tuple[Dict[str, Tensor], List[Dict[str, Tensor]]]:
+        """The ``<prefix>.*`` tensors of an ``AttentionEncoderOutputPooler`` of width ``width`` with
+        ``self.config.num_decoder_layers`` layers, in the engine's layout: ``pooler_q0``, ``proj_w`` and, when the
+        projection has a bias, ``proj_b``; and one ``SbPoolerLayerWeights`` dict per decoder layer."""
+        bf, f32 = self._bf16, self._f32
+        # the single decoder input: TransformerEmbeddingFrontend of token bos_idx = embed[bos_idx] * sqrt(width) + the
+        # sinusoid of position 0, [sin 0 ... | cos 0 ...] = [0 ... | 1 ...]  [fs2]
+        pos0 = torch.cat([torch.zeros(width // 2), torch.ones(width - width // 2)])
+        top = {"pooler_q0": f32(sd[f"{prefix}.decoder_frontend.embed.weight"][bos_idx].float() * math.sqrt(width) + pos0),
+               "proj_w": bf(sd[f"{prefix}.projection_out.weight"])}
+        if f"{prefix}.projection_out.bias" in sd:
+            top["proj_b"] = f32(sd[f"{prefix}.projection_out.bias"])
+        layers = []
+        for i in range(self.config.num_decoder_layers):
+            p = f"{prefix}.decoder.layers.{i}."
+            sa, ca = p + "self_attn.", p + "encoder_decoder_attn."
+            layers.append({
+                "sa_wv": bf(sd[sa + "v_proj.weight"]), "sa_bv": f32(sd[sa + "v_proj.bias"]),
+                "sa_wo": bf(sd[sa + "output_proj.weight"]), "sa_bo": f32(sd[sa + "output_proj.bias"]),
+                "sa_ln_g": f32(sd[p + "self_attn_layer_norm.weight"]), "sa_ln_b": f32(sd[p + "self_attn_layer_norm.bias"]),
+                "ca_wq": bf(sd[ca + "q_proj.weight"]), "ca_bq": f32(sd[ca + "q_proj.bias"]),
+                "ca_wkv": bf(torch.cat([sd[ca + "k_proj.weight"], sd[ca + "v_proj.weight"]], 0)),
+                "ca_bkv": f32(torch.cat([sd[ca + "k_proj.bias"], sd[ca + "v_proj.bias"]], 0)),
+                "ca_wo": bf(sd[ca + "output_proj.weight"]), "ca_bo": f32(sd[ca + "output_proj.bias"]),
+                "ca_ln_g": f32(sd[p + "encoder_decoder_attn_layer_norm.weight"]),
+                "ca_ln_b": f32(sd[p + "encoder_decoder_attn_layer_norm.bias"]),
+                "w1": bf(sd[p + "ffn.inner_proj.weight"]), "b1": f32(sd[p + "ffn.inner_proj.bias"]),
+                "w2": bf(sd[p + "ffn.output_proj.weight"]), "b2": f32(sd[p + "ffn.output_proj.bias"]),
+                "ffn_ln_g": f32(sd[p + "ffn_layer_norm.weight"]), "ffn_ln_b": f32(sd[p + "ffn_layer_norm.bias"]),
+            })
+        return top, layers
 
     def _create(self, cfg: C.Structure, weights: C.Structure) -> None:
         name = f"sb_{self._abi}_create"

@@ -1,6 +1,7 @@
 // SONAR speech encoder on sm_90a (BASELINE.json config 3; SURVEY §8 rows a11/a12, App. B.2/B.3):
 //   w2v-BERT frontend (stack 2 fbank frames -> LN(160) -> Linear 160->1024)
-//   -> 24 Conformer blocks -> model.layer_norm -> attention pooler (1 BOS query, POST-LN decoder layers) -> [B,1024]
+//   -> 24 Conformer blocks -> model.layer_norm -> attention pooler (1 BOS query, POST-LN decoder layers;
+//   AttentionPooler of latent_attention.cu, shared with the text encoder) -> [B,1024]
 // following SonarSpeechEncoderModel.forward (sonar/models/sonar_speech/model.py:59-77), factory.py:53-152,
 // nn/encoder_pooler.py:70-83; parameter names per sonar_speech/handler.py:63-100.
 //
@@ -474,74 +475,6 @@ glu_dwconv_kernel(const __nv_bfloat16* __restrict__ g, const int32_t* __restrict
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// pooler cross-attention: ONE query per utterance; kv bf16 [T, 2D] (k | v); one warp per (utterance, head)
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128)
-pool_attention_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kv,
-                      const int32_t* __restrict__ cu, int H, __nv_bfloat16* __restrict__ out) {
-  const int b = blockIdx.x;
-  const int h = blockIdx.y * 4 + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (h >= H) return;
-  const int D = H * 64;
-  const int start = cu[b], len = cu[b + 1] - start;
-  float qv[64];
-  {
-    const __nv_bfloat16* qr = q + (long long)b * D + h * 64;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const uint4 u = *reinterpret_cast<const uint4*>(qr + c * 8);
-      const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const __nv_bfloat162 t = *reinterpret_cast<const __nv_bfloat162*>(&w[e]);
-        qv[c * 8 + 2 * e] = __low2float(t);
-        qv[c * 8 + 2 * e + 1] = __high2float(t);
-      }
-    }
-  }
-  const float sl2 = 0.125f * 1.4426950408889634f;
-  float m = -CUDART_INF_F, l = 0.f, a0 = 0.f, a1 = 0.f;
-  for (int k0 = 0; k0 < len; k0 += 32) {
-    const int key = k0 + lane;
-    float s = -CUDART_INF_F;
-    if (key < len) {
-      const uint4* kp = reinterpret_cast<const uint4*>(kv + (long long)(start + key) * 2 * D + h * 64);
-      float d0 = 0.f, d1 = 0.f;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const uint4 u = kp[c];
-        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const __nv_bfloat162 t = *reinterpret_cast<const __nv_bfloat162*>(&w[e]);
-          d0 = fmaf(qv[c * 8 + 2 * e], __low2float(t), d0);
-          d1 = fmaf(qv[c * 8 + 2 * e + 1], __high2float(t), d1);
-        }
-      }
-      s = d0 + d1;
-    }
-    const float mn = fmaxf(m, warp_max(s));
-    const float corr = exp2f((m - mn) * sl2);
-    const float p = exp2f((s - mn) * sl2);
-    l = l * corr + warp_sum(p);
-    a0 *= corr;
-    a1 *= corr;
-    m = mn;
-    const int cnt = min(32, len - k0);
-    for (int j = 0; j < cnt; ++j) {
-      const float pj = __shfl_sync(0xffffffffu, p, j);
-      const __nv_bfloat162 vv =
-          *reinterpret_cast<const __nv_bfloat162*>(kv + (long long)(start + k0 + j) * 2 * D + D + h * 64 + lane * 2);
-      a0 = fmaf(pj, __low2float(vv), a0);
-      a1 = fmaf(pj, __high2float(vv), a1);
-    }
-  }
-  const float inv = (len > 0) ? 1.0f / l : 0.f;
-  *reinterpret_cast<uint32_t*>(out + (long long)b * D + h * 64 + lane * 2) = pack_bf16x2(a0 * inv, a1 * inv);
-}
-
 }  // namespace
 }  // namespace sb
 
@@ -551,7 +484,7 @@ struct SbSpeechEncoder {
   SbSpeechConfig cfg;
   SbSpeechWeights w;
   std::vector<SbConformerLayerWeights> layers;
-  std::vector<SbPoolerLayerWeights> pool;
+  AttentionPooler pooler;
   int num_sms;
 };
 
@@ -566,18 +499,14 @@ struct SpWs {
   float* vp;            // [H,Npad]
   __nv_bfloat16* qu;    // [T,D]
   __nv_bfloat16* qv;    // [T,D]
-  __nv_bfloat16* e;     // [T,D] pooler memory
-  float* px;            // [B,D]
-  __nv_bfloat16* ph;    // [B,D]
-  __nv_bfloat16* pt;    // [B,max(Fp,D)]
-  __nv_bfloat16* pq;    // [B,D]
+  AttentionPooler::Ws pool;
   size_t bytes;
 };
 
 int npad_of(int smax) { return ((2 * smax - 1) + 255) / 256 * 256; }
 
 SpWs carve_sp(const SbSpeechEncoder* e, int B, long long T, int smax, void* base) {
-  const size_t D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, Fp = e->cfg.pooler_ffn_inner_dim, H = e->cfg.num_heads;
+  const size_t D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, H = e->cfg.num_heads;
   const size_t np = npad_of(smax);
   size_t wide = F > 3 * D ? F : 3 * D;
   Carver c(base);
@@ -591,11 +520,7 @@ SpWs carve_sp(const SbSpeechEncoder* e, int B, long long T, int smax, void* base
   w.vp = c.take<float>(H * np * 4);
   w.qu = c.take<__nv_bfloat16>(t * D * 2);  // bf16(q + u), bf16(q + v): A operands of the wgmma attention
   w.qv = c.take<__nv_bfloat16>(t * D * 2);
-  w.e = c.take<__nv_bfloat16>(t * D * 2);
-  w.px = c.take<float>((size_t)B * D * 4);
-  w.ph = c.take<__nv_bfloat16>((size_t)B * D * 2);
-  w.pt = c.take<__nv_bfloat16>((size_t)B * (Fp > D ? Fp : D) * 2);
-  w.pq = c.take<__nv_bfloat16>((size_t)B * D * 2);
+  w.pool = e->pooler.take(c, (size_t)B);
   w.bytes = c.off;
   return w;
 }
@@ -615,18 +540,13 @@ int sb_speech_encoder_create(const SbSpeechConfig* cfg, const SbSpeechWeights* w
     return SB_ERR_INVALID;
   }
   if (!w->front_ln_g || !w->front_ln_b || !w->front_w || !w->front_b || !w->final_ln_g || !w->final_ln_b ||
-      !w->pooler_q0 || !w->proj_w || !w->zeros || (cfg->num_layers && !w->layers) || (cfg->pooler_layers && !w->pooler)) {
+      !w->zeros || (cfg->num_layers && !w->layers)) {
     set_last_error("sb_speech_encoder_create: missing weight pointer");
     return SB_ERR_INVALID;
   }
   for (int i = 0; i < cfg->num_layers; ++i)
     if (has_null_pointer(w->layers[i])) {
       set_last_error("sb_speech_encoder_create: conformer layer %d has a null weight pointer", i);
-      return SB_ERR_INVALID;
-    }
-  for (int i = 0; i < cfg->pooler_layers; ++i)
-    if (has_null_pointer(w->pooler[i])) {
-      set_last_error("sb_speech_encoder_create: pooler layer %d has a null weight pointer", i);
       return SB_ERR_INVALID;
     }
   int num_sms = 0;
@@ -636,13 +556,22 @@ int sb_speech_encoder_create(const SbSpeechConfig* cfg, const SbSpeechWeights* w
   e->cfg = *cfg;
   e->w = *w;
   e->layers.assign(w->layers, w->layers + cfg->num_layers);
-  e->pool.assign(w->pooler, w->pooler + cfg->pooler_layers);
   e->num_sms = num_sms;
+  // the projection has no bias: zeros; every GEMM of this engine may take the weight-streaming path
+  if (int rc = e->pooler.create("sb_speech_encoder_create", w->pooler, cfg->pooler_layers, w->pooler_q0, w->proj_w, w->zeros,
+                                D, D, cfg->pooler_ffn_inner_dim, cfg->ln_eps, num_sms, 2, 1)) {
+    sb_speech_encoder_destroy(e);
+    return rc;
+  }
   *out = e;
   return SB_OK;
 }
 
-void sb_speech_encoder_destroy(SbSpeechEncoder* e) { delete e; }
+void sb_speech_encoder_destroy(SbSpeechEncoder* e) {
+  if (!e) return;
+  e->pooler.destroy();
+  delete e;
+}
 
 int sb_speech_encoder_workspace_bytes(const SbSpeechEncoder* e, int32_t B, int64_t total_positions, int32_t max_positions,
                                       size_t* bytes) {
@@ -682,7 +611,7 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
                           [&](void* p) { return carve_sp(e, B, T, smax, p); });
   if (rc) return rc;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  const int D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, H = e->cfg.num_heads, Fp = e->cfg.pooler_ffn_inner_dim;
+  const int D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, H = e->cfg.num_heads;
   const float eps = e->cfg.ln_eps;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
@@ -692,7 +621,7 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
   CUtensorMap tm_qkv, tm_p;
   if ((rc = make_tmap_2d(&tm_qkv, w.big, 2, T, 3ll * D, 3ll * D, 64, 64))) return rc;
   if ((rc = make_tmap_2d(&tm_p, w.p, 2, Npad, D, D, 64, 64))) return rc;
-  // every GEMM may take the weight-streaming path (the pooler's B rows)
+  // every GEMM may take the weight-streaming path (as the pooler's do)
   auto gemm = [&](const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int fp32,
                   const float* bias, int M, int N, int K, int epi) {
     GemmArgs g = gemm_args(A, lda, W, ldw, C, ldc, fp32, bias, M, N, K, epi, e->num_sms);
@@ -748,29 +677,9 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
     if ((rc = layernorm_dual(w.x, L.ln_g, L.ln_b, eps, w.x, nullptr, T, D, stream))) return rc;
   }
   // ---- model.layer_norm (fp32 in place, bf16 copy = pooler memory) ----
-  if ((rc = layernorm_dual(w.x, e->w.final_ln_g, e->w.final_ln_b, eps, w.x, w.e, T, D, stream))) return rc;
+  if ((rc = layernorm_dual(w.x, e->w.final_ln_g, e->w.final_ln_b, eps, w.x, w.h, T, D, stream))) return rc;
   if (encoded_packed) SB_CUDA_CHECK(cudaMemcpyAsync(encoded_packed, w.x, sizeof(float) * (size_t)T * D, cudaMemcpyDeviceToDevice, stream));
-  // ---- attention pooler ----
-  if ((rc = broadcast_rows(e->w.pooler_q0, w.px, w.ph, B, D, stream))) return rc;
-  for (int li = 0; li < e->cfg.pooler_layers; ++li) {
-    const SbPoolerLayerWeights& P = e->pool[li];
-    // self-attention over the single query token == Wo(Wv x + bv) + bo
-    if ((rc = gemm(w.ph, D, P.sa_wv, D, w.pt, D, 0, P.sa_bv, B, D, D, EPI_BIAS))) return rc;
-    if ((rc = gemm(w.pt, D, P.sa_wo, D, w.px, D, 1, P.sa_bo, B, D, D, EPI_BIAS_RESIDUAL))) return rc;
-    if ((rc = layernorm_dual(w.px, P.sa_ln_g, P.sa_ln_b, eps, w.px, w.ph, B, D, stream))) return rc;
-    // cross-attention over the utterance
-    if ((rc = gemm(w.ph, D, P.ca_wq, D, w.pq, D, 0, P.ca_bq, B, D, D, EPI_BIAS))) return rc;
-    if ((rc = gemm(w.e, D, P.ca_wkv, D, w.big, 2 * D, 0, P.ca_bkv, (int)T, 2 * D, D, EPI_BIAS))) return rc;
-    pool_attention_kernel<<<dim3((unsigned)B, (unsigned)((H + 3) / 4)), 128, 0, stream>>>(w.pq, w.big, cu_dev, H, w.pt);
-    SB_CUDA_CHECK(cudaGetLastError());
-    if ((rc = gemm(w.pt, D, P.ca_wo, D, w.px, D, 1, P.ca_bo, B, D, D, EPI_BIAS_RESIDUAL))) return rc;
-    if ((rc = layernorm_dual(w.px, P.ca_ln_g, P.ca_ln_b, eps, w.px, w.ph, B, D, stream))) return rc;
-    // ReLU FFN
-    if ((rc = gemm(w.ph, D, P.w1, D, w.pt, Fp, 0, P.b1, B, Fp, D, EPI_BIAS_RELU))) return rc;
-    if ((rc = gemm(w.pt, Fp, P.w2, Fp, w.px, D, 1, P.b2, B, D, Fp, EPI_BIAS_RESIDUAL))) return rc;
-    if ((rc = layernorm_dual(w.px, P.ffn_ln_g, P.ffn_ln_b, eps, w.px, w.ph, B, D, stream))) return rc;
-  }
-  return gemm(w.ph, D, e->w.proj_w, D, out, D, 1, e->w.zeros, B, D, D, EPI_BIAS);
+  return e->pooler.forward(w.pool, w.h, cu_dev, B, out, stream);
 }
 
 }  // extern "C"

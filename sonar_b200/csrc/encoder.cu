@@ -21,10 +21,7 @@
 // the classic schedule: separate LayerNorm kernels, residual adds by TMA reduce-add, 7 launches per layer.
 //
 // Attention pooling (SB_POOL_ATTENTION, factory.py:155-226): the final LayerNorm writes x in place and its bf16 copy h, the
-// pooler's memory; then one query row per sentence (px fp32 / ph bf16 [B, E]) runs the POST-LN decoder layers
-//   [ self-attention over itself = Wo (Wv x + bv) + bo -> LN -> absorbed query GEMM (qt [B, Hd*D]) -> latent
-//     cross-attention over h (latent_attention.cu) -> absorbed output GEMM (+residual) -> LN -> ReLU FFN -> LN ]
-// and projection_out (+bias) writes out [B, E].  The absorbed weights are prepared at create in device memory the handle owns.
+// memory of the attention pooler (AttentionPooler, latent_attention.cu), which writes out [B, E].
 
 #include "../../include/sonar_b200.h"
 #include <stdlib.h>
@@ -73,12 +70,7 @@ struct Workspace {
   __nv_bfloat16* h;
   __nv_bfloat16* qkv;
   __nv_bfloat16* f;
-  // attention pooling only
-  float* px;           // [B, max(D, E)] fp32 pooler state (its first B*D floats are scratch for the `encoded` scatter)
-  __nv_bfloat16* ph;   // [B, E] bf16 copy of px
-  __nv_bfloat16* pt;   // [B, max(F_pool, E)]
-  __nv_bfloat16* qt;   // [B, Hd*D] absorbed queries
-  __nv_bfloat16* u;    // [B, Hd*D] latent attention output
+  AttentionPooler::Ws pool;  // attention pooling only
   size_t bytes;
 };
 
@@ -95,13 +87,6 @@ struct FoldedLayer {  // LnFold weights of one layer (device memory owned by the
   float* b1 = nullptr;
 };
 
-struct AbsorbedPoolerLayer {  // cross-attention weights of one pooler layer on the latent form (owned by the handle)
-  __nv_bfloat16* wqk = nullptr;  // [Hd*D, E]
-  float* bqk = nullptr;          // [Hd*D]
-  __nv_bfloat16* wvo = nullptr;  // [E, Hd*D]
-  float* bvo = nullptr;          // [E]
-};
-
 struct SbEncoder {
   SbEncoderConfig cfg;
   int out_dim;  // width of `out`: embedding_dim with attention pooling, model_dim otherwise
@@ -113,12 +98,7 @@ struct SbEncoder {
   const float* final_ln_g;
   const float* final_ln_b;
   std::vector<SbLayerWeights> layers;
-  std::vector<SbPoolerLayerWeights> pool;
-  std::vector<AbsorbedPoolerLayer> absorbed;
-  void* absorb_pool = nullptr;  // one allocation behind all AbsorbedPoolerLayer pointers
-  const float* pooler_q0 = nullptr;
-  const void* proj_w = nullptr;
-  const float* proj_b = nullptr;
+  AttentionPooler pooler;  // attention pooling only
   int num_sms;
   // pinned staging ring for cu_seqlens
   static constexpr int kSlots = 8;
@@ -142,58 +122,16 @@ static Workspace carve(const SbEncoder* e, int32_t max_batch, int64_t max_tokens
   w.h = c.take<__nv_bfloat16>(T * D * 2);
   w.qkv = c.take<__nv_bfloat16>(T * 3 * D * 2);
   w.f = c.take<__nv_bfloat16>(T * F * 2);
-  w.px = nullptr; w.ph = w.pt = w.qt = w.u = nullptr;
-  if (e->cfg.pooling == SB_POOL_ATTENTION) {
-    const size_t B = (size_t)max_batch, E = e->cfg.embedding_dim, Fp = e->cfg.pooler_ffn_inner_dim;
-    const size_t HdD = (size_t)e->cfg.pooler_heads * D;
-    w.px = c.take<float>(B * (D > E ? D : E) * 4);
-    w.ph = c.take<__nv_bfloat16>(B * E * 2);
-    w.pt = c.take<__nv_bfloat16>(B * (Fp > E ? Fp : E) * 2);
-    w.qt = c.take<__nv_bfloat16>(B * HdD * 2);
-    w.u = c.take<__nv_bfloat16>(B * HdD * 2);
-  }
+  w.pool = {};
+  if (e->cfg.pooling == SB_POOL_ATTENTION) w.pool = e->pooler.take(c, (size_t)max_batch);
   w.bytes = c.off;
   return w;
-}
-
-// The attention pooler (SB_POOL_ATTENTION) over the memory w.h [T, D]: writes out [B, E] fp32.
-static int attention_pooler(const SbEncoder* e, const Workspace& w, int B, float* out, cudaStream_t stream) {
-  const int D = e->cfg.model_dim, E = e->cfg.embedding_dim, Hd = e->cfg.pooler_heads, Fp = e->cfg.pooler_ffn_inner_dim;
-  const int HdD = Hd * D;
-  const float eps = e->cfg.ln_eps;
-  const int cta_group = (e->cfg.cta_group == 1) ? 1 : 2;
-  auto gemm = [&](const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int fp32,
-                  const float* bias, int N, int K, int epi) {
-    GemmArgs g = gemm_args(A, lda, W, ldw, C, ldc, fp32, bias, B, N, K, epi, e->num_sms);
-    g.cta_group = cta_group;
-    return gemm_bf16(g, stream);
-  };
-  int rc;
-  if ((rc = broadcast_rows(e->pooler_q0, w.px, w.ph, B, E, stream))) return rc;
-  for (int li = 0; li < e->cfg.pooler_layers; ++li) {
-    const SbPoolerLayerWeights& P = e->pool[li];
-    const AbsorbedPoolerLayer& A = e->absorbed[li];
-    // self-attention over the single query token == Wo(Wv x + bv) + bo
-    if ((rc = gemm(w.ph, E, P.sa_wv, E, w.pt, E, 0, P.sa_bv, E, E, EPI_BIAS))) return rc;
-    if ((rc = gemm(w.pt, E, P.sa_wo, E, w.px, E, 1, P.sa_bo, E, E, EPI_BIAS_RESIDUAL))) return rc;
-    if ((rc = layernorm_dual(w.px, P.sa_ln_g, P.sa_ln_b, eps, w.px, w.ph, B, E, stream))) return rc;
-    // cross-attention over the sentence on the absorbed form
-    if ((rc = gemm(w.ph, E, A.wqk, E, w.qt, HdD, 0, A.bqk, HdD, E, EPI_BIAS))) return rc;
-    if ((rc = pool_latent_attention(w.qt, w.h, w.cu, B, Hd, D, w.u, stream))) return rc;
-    if ((rc = gemm(w.u, HdD, A.wvo, HdD, w.px, E, 1, A.bvo, E, HdD, EPI_BIAS_RESIDUAL))) return rc;
-    if ((rc = layernorm_dual(w.px, P.ca_ln_g, P.ca_ln_b, eps, w.px, w.ph, B, E, stream))) return rc;
-    // ReLU FFN
-    if ((rc = gemm(w.ph, E, P.w1, E, w.pt, Fp, 0, P.b1, Fp, E, EPI_BIAS_RELU))) return rc;
-    if ((rc = gemm(w.pt, Fp, P.w2, Fp, w.px, E, 1, P.b2, E, Fp, EPI_BIAS_RESIDUAL))) return rc;
-    if ((rc = layernorm_dual(w.px, P.ffn_ln_g, P.ffn_ln_b, eps, w.px, w.ph, B, E, stream))) return rc;
-  }
-  return gemm(w.ph, E, e->proj_w, E, out, E, 1, e->proj_b, E, E, EPI_BIAS);
 }
 
 extern "C" {
 
 const char* sb_last_error(void) { return g_err; }
-int sb_version(void) { return 105; }
+int sb_version(void) { return 106; }
 
 int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbEncoder** out) {
   if (!cfg || !w || !out) { set_last_error("sb_encoder_create: null argument"); return SB_ERR_INVALID; }
@@ -230,15 +168,6 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
                      "(got %d, %d)", cfg->pooler_layers, cfg->pooler_ffn_inner_dim);
       return SB_ERR_INVALID;
     }
-    if (!w->pooler_q0 || !w->proj_w || !w->proj_b || !w->pooler) {
-      set_last_error("sb_encoder_create: attention pooling needs pooler_q0, proj_w, proj_b and pooler");
-      return SB_ERR_INVALID;
-    }
-    for (int i = 0; i < cfg->pooler_layers; ++i)
-      if (has_null_pointer(w->pooler[i])) {
-        set_last_error("sb_encoder_create: pooler layer %d has a null weight pointer", i);
-        return SB_ERR_INVALID;
-      }
   } else if (E != 0 && E != D) {
     set_last_error("sb_encoder_create: embedding_dim (%d) != model_dim (%d) needs attention pooling", E, D);
     return SB_ERR_INVALID;
@@ -263,12 +192,6 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
   e->final_ln_b = w->final_ln_b;
   e->layers.assign(w->layers, w->layers + cfg->num_layers);
   e->out_dim = attn_pool ? E : D;
-  if (attn_pool) {
-    e->pool.assign(w->pooler, w->pooler + cfg->pooler_layers);
-    e->pooler_q0 = w->pooler_q0;
-    e->proj_w = w->proj_w;
-    e->proj_b = w->proj_b;
-  }
   e->num_sms = cfg->num_sms > 0 ? cfg->num_sms : num_sms;
   for (int i = 0; i < SbEncoder::kSlots; ++i) e->ev_ok[i] = false;
   if (cudaMallocHost(reinterpret_cast<void**>(&e->pinned), sizeof(int32_t) * SbEncoder::kSlots * SbEncoder::kSlotInts) !=
@@ -324,38 +247,9 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
     }
   }
   if (attn_pool) {
-    // absorbed cross-attention weights of every pooler layer (latent_attention.cu); the caller's weights are not modified
-    const size_t HdD = (size_t)cfg->pooler_heads * D, E_ = E;
-    auto carve_absorbed = [&](void* base) {
-      Carver c(base);
-      for (AbsorbedPoolerLayer& a : e->absorbed) {
-        a.wqk = c.take<__nv_bfloat16>(HdD * E_ * 2, 256);
-        a.bqk = c.take<float>(HdD * 4, 256);
-        a.wvo = c.take<__nv_bfloat16>(E_ * HdD * 2, 256);
-        a.bvo = c.take<float>(E_ * 4, 256);
-      }
-      return c.off;
-    };
-    e->absorbed.resize(cfg->pooler_layers);
-    const size_t pool_bytes = carve_absorbed(nullptr);
-    if (cudaMalloc(&e->absorb_pool, pool_bytes) != cudaSuccess) {
-      set_last_error("sb_encoder_create: cudaMalloc of %zu bytes for the absorbed pooler weights failed", pool_bytes);
-      sb_encoder_destroy(e);
-      return SB_ERR_CUDA;
-    }
-    carve_absorbed(e->absorb_pool);
-    for (int i = 0; i < cfg->pooler_layers; ++i) {
-      const AbsorbedPoolerLayer& a = e->absorbed[i];
-      if (int rc = absorb_pooler_weights(e->pool[i], D, E, a.wqk, a.bqk, a.wvo, a.bvo, nullptr)) {
-        sb_encoder_destroy(e);
-        return rc;
-      }
-    }
-    if (cudaDeviceSynchronize() != cudaSuccess) {
-      set_last_error("sb_encoder_create: absorbing the pooler weights failed: %s", cudaGetErrorString(cudaGetLastError()));
-      sb_encoder_destroy(e);
-      return SB_ERR_CUDA;
-    }
+    const int rc = e->pooler.create("sb_encoder_create", w->pooler, cfg->pooler_layers, w->pooler_q0, w->proj_w, w->proj_b,
+                                    D, E, cfg->pooler_ffn_inner_dim, cfg->ln_eps, e->num_sms, cfg->cta_group == 1 ? 1 : 2, 0);
+    if (rc) { sb_encoder_destroy(e); return rc; }
   }
   for (int i = 0; i < SbEncoder::kSlots; ++i) {
     if (cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming) != cudaSuccess) {
@@ -375,7 +269,7 @@ void sb_encoder_destroy(SbEncoder* e) {
     if (e->ev_ok[i]) cudaEventDestroy(e->ev[i]);
   if (e->pinned) cudaFreeHost(e->pinned);
   if (e->fold_pool) cudaFree(e->fold_pool);
-  if (e->absorb_pool) cudaFree(e->absorb_pool);
+  e->pooler.destroy();
   if (e->err_flag) cudaFree(e->err_flag);
   delete e;
 }
@@ -429,7 +323,7 @@ int sb_encoder_forward(SbEncoder* e, const int64_t* ids, int64_t ids_row_stride,
       return SB_OK;
     }
     if (encoded) SB_CUDA_CHECK(cudaMemsetAsync(encoded, 0, sizeof(float) * (size_t)B * S * D, stream));
-    return attention_pooler(e, w, B, out, stream);
+    return e->pooler.forward(w.pool, w.h, w.cu, B, out, stream);
   }
 
   const bool fold = e->cfg.ln_fold != 0 && e->cfg.num_layers > 0;  // LN1 (attention block) folded into FFN2 -> QKV
@@ -490,8 +384,9 @@ int sb_encoder_forward(SbEncoder* e, const int64_t* ids, int64_t ids_row_stride,
   // final LayerNorm in place + its bf16 copy (the pooler's memory); `encoded` is scattered from the normalised rows
   if ((rc = layernorm_dual(w.x, e->final_ln_g, e->final_ln_b, e->cfg.ln_eps, w.x, w.h, T, D, stream))) return rc;
   if (encoded)
-    if ((rc = ln_pool(w.x, w.cu, B, D, nullptr, nullptr, e->cfg.ln_eps, 0, POOL_LAST, w.px, encoded, S, stream))) return rc;
-  return attention_pooler(e, w, B, out, stream);
+    if ((rc = ln_pool(w.x, w.cu, B, D, nullptr, nullptr, e->cfg.ln_eps, 0, POOL_LAST, w.pool.px, encoded, S, stream)))
+      return rc;
+  return e->pooler.forward(w.pool, w.h, w.cu, B, out, stream);
 }
 
 int sb_encoder_forward_host(SbEncoder* e, const int64_t* ids_host, const int32_t* seq_lens_host, int32_t B,

@@ -1,6 +1,8 @@
-// Single-query latent cross-attention of the text encoder's attention pooler, and the create-time weight absorption
-// behind it (SbEncoderConfig.pooling = SB_POOL_ATTENTION; reference: SonarTextEncoderFactory.create_attention_pooler,
-// sonar/models/sonar_text/factory.py:155-226, i.e. fairseq2's encoder-decoder attention with ONE decoder position).
+// The attention pooler of the text and speech encoders (AttentionPooler, sonar_b200_internal.h): its single-query latent
+// cross-attention, the create-time weight absorption behind it and the layer loop around it (reference:
+// AttentionEncoderOutputPooler, sonar/nn/encoder_pooler.py:47-89, built by SonarTextEncoderFactory.create_attention_pooler,
+// sonar/models/sonar_text/factory.py:155-226, and by the speech factory; fairseq2's encoder-decoder attention with ONE
+// decoder position).
 //
 // For head h (head dim 64, scale 1/8), memory row m_t (final-LayerNormed token state, width D) and pooler query q:
 //   score_t = q_h . (W_k,h m_t + b_k,h) / 8 = (W_k,h^T q_h) . m_t / 8 + const      (softmax cancels the constant)
@@ -253,8 +255,10 @@ int pool_latent_attention(const __nv_bfloat16* qt, const __nv_bfloat16* mem, con
   }
 }
 
-int absorb_pooler_weights(const SbPoolerLayerWeights& P, int D, int E, __nv_bfloat16* wqk, float* bqk, __nv_bfloat16* wvo,
-                          float* bvo, cudaStream_t stream) {
+// Absorbs the cross-attention projections of one pooler layer (kv width D, pooler width E = 64 Hd) into the
+// AttentionPooler::Layer weights wqk / bqk / wvo / bvo.
+static int absorb_pooler_weights(const SbPoolerLayerWeights& P, int D, int E, __nv_bfloat16* wqk, float* bqk,
+                                 __nv_bfloat16* wvo, float* bvo, cudaStream_t stream) {
   const int Hd = E / 64;
   const auto* wq = reinterpret_cast<const __nv_bfloat16*>(P.ca_wq);
   const auto* wk = reinterpret_cast<const __nv_bfloat16*>(P.ca_wkv);
@@ -272,6 +276,98 @@ int absorb_pooler_weights(const SbPoolerLayerWeights& P, int D, int E, __nv_bflo
   absorb_bias_kernel<<<(unsigned)((E + 255) / 256), 256, 0, stream>>>(wo, 1, E, P.ca_bkv + E, E, E, 1, P.ca_bo, bvo);
   SB_CUDA_CHECK(cudaGetLastError());
   return 0;
+}
+
+int AttentionPooler::create(const char* who, const SbPoolerLayerWeights* w, int num_layers, const float* q0,
+                            const void* proj_w, const float* proj_b, int D, int E, int F, float eps, int num_sms,
+                            int cta_group, int allow_skinny) {
+  if (!q0 || !proj_w || !proj_b || (num_layers > 0 && !w)) {
+    set_last_error("%s: attention pooling needs pooler_q0, proj_w, proj_b and pooler", who);
+    return SB_ERR_INVALID;
+  }
+  for (int i = 0; i < num_layers; ++i)
+    if (has_null_pointer(w[i])) {
+      set_last_error("%s: pooler layer %d has a null weight pointer", who, i);
+      return SB_ERR_INVALID;
+    }
+  this->q0 = q0; this->proj_w = proj_w; this->proj_b = proj_b;
+  this->D = D; this->E = E; this->F = F; this->eps = eps;
+  this->num_sms = num_sms; this->cta_group = cta_group; this->allow_skinny = allow_skinny;
+  layers.resize(num_layers);
+  for (int i = 0; i < num_layers; ++i) layers[i].w = w[i];
+  // absorbed cross-attention weights of every layer; the caller's weights are not modified
+  const size_t HdD = (size_t)(E / 64) * D, Es = E;
+  auto carve = [&](void* base) {
+    Carver c(base);
+    for (Layer& l : layers) {
+      l.wqk = c.take<__nv_bfloat16>(HdD * Es * 2, 256);
+      l.bqk = c.take<float>(HdD * 4, 256);
+      l.wvo = c.take<__nv_bfloat16>(Es * HdD * 2, 256);
+      l.bvo = c.take<float>(Es * 4, 256);
+    }
+    return c.off;
+  };
+  const size_t bytes = carve(nullptr);
+  if (bytes && cudaMalloc(&absorbed, bytes) != cudaSuccess) {
+    absorbed = nullptr;
+    set_last_error("%s: cudaMalloc of %zu bytes for the absorbed pooler weights failed", who, bytes);
+    return SB_ERR_CUDA;
+  }
+  carve(absorbed);
+  for (const Layer& l : layers)
+    if (int rc = absorb_pooler_weights(l.w, D, E, l.wqk, l.bqk, l.wvo, l.bvo, nullptr)) return rc;
+  if (cudaDeviceSynchronize() != cudaSuccess) {
+    set_last_error("%s: absorbing the pooler weights failed: %s", who, cudaGetErrorString(cudaGetLastError()));
+    return SB_ERR_CUDA;
+  }
+  return SB_OK;
+}
+
+void AttentionPooler::destroy() {
+  if (absorbed) cudaFree(absorbed);
+  absorbed = nullptr;
+}
+
+AttentionPooler::Ws AttentionPooler::take(Carver& c, size_t B) const {
+  const size_t Ds = D, Es = E, Fs = F, HdD = (size_t)(E / 64) * D;
+  Ws w;
+  w.px = c.take<float>(B * (Ds > Es ? Ds : Es) * 4);
+  w.ph = c.take<__nv_bfloat16>(B * Es * 2);
+  w.pt = c.take<__nv_bfloat16>(B * (Fs > Es ? Fs : Es) * 2);
+  w.qt = c.take<__nv_bfloat16>(B * HdD * 2);
+  w.u = c.take<__nv_bfloat16>(B * HdD * 2);
+  return w;
+}
+
+int AttentionPooler::forward(const Ws& w, const __nv_bfloat16* mem, const int32_t* cu_seqlens, int B, float* out,
+                             cudaStream_t stream) const {
+  const int Hd = E / 64, HdD = Hd * D;
+  auto gemm = [&](const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int fp32,
+                  const float* bias, int N, int K, int epi) {
+    GemmArgs g = gemm_args(A, lda, W, ldw, C, ldc, fp32, bias, B, N, K, epi, num_sms);
+    g.cta_group = cta_group;
+    g.allow_skinny = allow_skinny;
+    return gemm_bf16(g, stream);
+  };
+  int rc;
+  if ((rc = broadcast_rows(q0, w.px, w.ph, B, E, stream))) return rc;
+  for (const Layer& l : layers) {
+    const SbPoolerLayerWeights& P = l.w;
+    // self-attention over the single query token == Wo(Wv x + bv) + bo
+    if ((rc = gemm(w.ph, E, P.sa_wv, E, w.pt, E, 0, P.sa_bv, E, E, EPI_BIAS))) return rc;
+    if ((rc = gemm(w.pt, E, P.sa_wo, E, w.px, E, 1, P.sa_bo, E, E, EPI_BIAS_RESIDUAL))) return rc;
+    if ((rc = layernorm_dual(w.px, P.sa_ln_g, P.sa_ln_b, eps, w.px, w.ph, B, E, stream))) return rc;
+    // cross-attention over the sequence on the absorbed form
+    if ((rc = gemm(w.ph, E, l.wqk, E, w.qt, HdD, 0, l.bqk, HdD, E, EPI_BIAS))) return rc;
+    if ((rc = pool_latent_attention(w.qt, mem, cu_seqlens, B, Hd, D, w.u, stream))) return rc;
+    if ((rc = gemm(w.u, HdD, l.wvo, HdD, w.px, E, 1, l.bvo, E, HdD, EPI_BIAS_RESIDUAL))) return rc;
+    if ((rc = layernorm_dual(w.px, P.ca_ln_g, P.ca_ln_b, eps, w.px, w.ph, B, E, stream))) return rc;
+    // ReLU FFN
+    if ((rc = gemm(w.ph, E, P.w1, E, w.pt, F, 0, P.b1, F, E, EPI_BIAS_RELU))) return rc;
+    if ((rc = gemm(w.pt, F, P.w2, F, w.px, E, 1, P.b2, E, F, EPI_BIAS_RESIDUAL))) return rc;
+    if ((rc = layernorm_dual(w.px, P.ffn_ln_g, P.ffn_ln_b, eps, w.px, w.ph, B, E, stream))) return rc;
+  }
+  return gemm(w.ph, E, proj_w, E, out, E, 1, proj_b, E, E, EPI_BIAS);
 }
 
 }  // namespace sb

@@ -10,6 +10,8 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <vector>
+
 namespace sb {
 
 // EPI_BIAS_ACCUM (internal): C += A.W^T + bias with the add done by TMA reduce-add at L2; chosen
@@ -226,17 +228,53 @@ int attention_relpos_tc(const __nv_bfloat16* qkv, const __nv_bfloat16* p, const 
 // x [B, D] fp32 and xb [B, D] bf16 = B copies of the fp32 row v [D] (the attention poolers' single query position)
 int broadcast_rows(const float* v, float* x, __nv_bfloat16* xb, int B, int D, cudaStream_t stream);
 
-// Text attention pooler (latent_attention.cu).  u [B, Hd, D] bf16 = softmax_t(qt[b, h, :] . mem[t, :] / 8) . mem over the
-// rows t of sentence b in the packed memory mem [T, D] bf16; qt [B, Hd, D] bf16; Hd <= 16; D in {256, 512, 768, 1024};
-// an empty sentence gives zeros.
+// Latent cross-attention of the attention pooler (latent_attention.cu).  u [B, Hd, D] bf16 = softmax_t(qt[b, h, :] .
+// mem[t, :] / 8) . mem over the rows t of sequence b in the packed memory mem [T, D] bf16; qt [B, Hd, D] bf16; Hd <= 16;
+// D in {256, 512, 768, 1024}; an empty sequence gives zeros.
 int pool_latent_attention(const __nv_bfloat16* qt, const __nv_bfloat16* mem, const int32_t* cu_seqlens, int B, int Hd, int D,
                           __nv_bfloat16* u, cudaStream_t stream);
-// Absorbs the cross-attention projections of one pooler layer (kv width D, pooler width E = 64 Hd) so that the layer runs
-// on pool_latent_attention: wqk [Hd*D, E] / bqk [Hd*D] map the pooler state to the absorbed queries
-// (qt_h = W_k,h^T (W_q,h x + b_q,h)); wvo [E, Hd*D] / bvo [E] map u to the attention output (W_o blockdiag(W_v,h) u +
-// W_o b_v + b_o).  The key bias drops out (softmax is shift-invariant).
-int absorb_pooler_weights(const SbPoolerLayerWeights& P, int D, int E, __nv_bfloat16* wqk, float* bqk, __nv_bfloat16* wvo,
-                          float* bvo, cudaStream_t stream);
+
+// The attention pooler of the text and speech encoders (latent_attention.cu; AttentionEncoderOutputPooler,
+// sonar/nn/encoder_pooler.py:47-89): one query row per sequence (px fp32 / ph bf16 [B, E], starting from q0) runs the
+// POST-LN decoder layers
+//   [ self-attention over itself = Wo (Wv x + bv) + bo -> LN -> absorbed query GEMM (qt [B, Hd*D]) -> latent
+//     cross-attention over the memory (pool_latent_attention) -> absorbed output GEMM (+residual) -> LN -> ReLU FFN -> LN ]
+// and projection_out (+bias) writes out [B, E] fp32.  Memory width D, pooler width E = 64 Hd (both multiples of 256,
+// <= 1024; the engines check that), FFN width F.  The GEMMs run with the owning engine's GEMM policy.
+struct AttentionPooler {
+  struct Layer {
+    SbPoolerLayerWeights w;          // the caller's weights (copied at create)
+    __nv_bfloat16* wqk = nullptr;    // [Hd*D, E]  absorbed W_k,h^T W_q,h: qt_h = W_k,h^T (W_q,h x + b_q,h)
+    float* bqk = nullptr;            // [Hd*D]
+    __nv_bfloat16* wvo = nullptr;    // [E, Hd*D]  absorbed W_o blockdiag(W_v,h)
+    float* bvo = nullptr;            // [E]        W_o b_v + b_o (the key bias drops out: softmax is shift-invariant)
+  };
+  struct Ws {  // the pooler's workspace buffers
+    float* px = nullptr;          // [B, max(D, E)] fp32 pooler state (the text encoder's `encoded` scatter uses its first B*D)
+    __nv_bfloat16* ph = nullptr;  // [B, E] bf16 copy of px
+    __nv_bfloat16* pt = nullptr;  // [B, max(F, E)]
+    __nv_bfloat16* qt = nullptr;  // [B, Hd*D] absorbed queries
+    __nv_bfloat16* u = nullptr;   // [B, Hd*D] latent attention output
+  };
+  std::vector<Layer> layers;
+  void* absorbed = nullptr;  // one device allocation behind every layer's absorbed weights
+  const float* q0 = nullptr;      // fp32 [E]
+  const void* proj_w = nullptr;   // bf16 [E, E]
+  const float* proj_b = nullptr;  // fp32 [E]
+  int D = 0, E = 0, F = 0;
+  float eps = 0.f;
+  int num_sms = 0, cta_group = 2, allow_skinny = 0;  // GEMM policy
+
+  // Checks the weight pointers, copies the layers and absorbs their cross-attention weights into one allocation of
+  // num_layers * (2 Hd D E * 2 + (Hd D + E) * 4) bytes, then synchronises the device.  Errors name `who`; on failure the
+  // caller still calls destroy().
+  int create(const char* who, const SbPoolerLayerWeights* w, int num_layers, const float* q0, const void* proj_w,
+             const float* proj_b, int D, int E, int F, float eps, int num_sms, int cta_group, int allow_skinny);
+  void destroy();
+  Ws take(Carver& c, size_t B) const;  // the next buffers of a workspace layout, for B sequences
+  // out [B, E] fp32 from the memory mem [T, D] bf16 packed by cu_seqlens [B + 1]
+  int forward(const Ws& w, const __nv_bfloat16* mem, const int32_t* cu_seqlens, int B, float* out, cudaStream_t stream) const;
+};
 
 // optional final LayerNorm + pooling over packed sequences -> out [B, D] fp32;
 // optionally also scatters the (normalised) rows to a padded [B, S, D] fp32 tensor.

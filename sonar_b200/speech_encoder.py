@@ -85,7 +85,7 @@ class B200SpeechEncoderModel(EngineModel):
         sd, d = state_dict, config.model_dim
         bf, f32 = self._bf16, self._f32
 
-        layers, pooler = [], []
+        layers = []
         for i in range(config.num_encoder_layers):
             p = f"encoder.layers.{i}."
             a = p + "self_attn."
@@ -111,36 +111,16 @@ class B200SpeechEncoderModel(EngineModel):
                 "ffn2_w2": bf(sd[p + "ffn2.output_proj.weight"].float() * 0.5), "ffn2_b2": f32(sd[p + "ffn2.output_proj.bias"].float() * 0.5),
                 "ln_g": f32(sd[p + "layer_norm.weight"]), "ln_b": f32(sd[p + "layer_norm.bias"]),
             })
-        for i in range(config.num_decoder_layers):
-            p = f"encoder_pooler.decoder.layers.{i}."
-            s_, c_ = p + "self_attn.", p + "encoder_decoder_attn."
-            pooler.append({
-                "sa_wv": bf(sd[s_ + "v_proj.weight"]), "sa_bv": f32(sd[s_ + "v_proj.bias"]),
-                "sa_wo": bf(sd[s_ + "output_proj.weight"]), "sa_bo": f32(sd[s_ + "output_proj.bias"]),
-                "sa_ln_g": f32(sd[p + "self_attn_layer_norm.weight"]), "sa_ln_b": f32(sd[p + "self_attn_layer_norm.bias"]),
-                "ca_wq": bf(sd[c_ + "q_proj.weight"]), "ca_bq": f32(sd[c_ + "q_proj.bias"]),
-                "ca_wkv": bf(torch.cat([sd[c_ + "k_proj.weight"], sd[c_ + "v_proj.weight"]], 0)),
-                "ca_bkv": f32(torch.cat([sd[c_ + "k_proj.bias"], sd[c_ + "v_proj.bias"]], 0)),
-                "ca_wo": bf(sd[c_ + "output_proj.weight"]), "ca_bo": f32(sd[c_ + "output_proj.bias"]),
-                "ca_ln_g": f32(sd[p + "encoder_decoder_attn_layer_norm.weight"]),
-                "ca_ln_b": f32(sd[p + "encoder_decoder_attn_layer_norm.bias"]),
-                "w1": bf(sd[p + "ffn.inner_proj.weight"]), "b1": f32(sd[p + "ffn.inner_proj.bias"]),
-                "w2": bf(sd[p + "ffn.output_proj.weight"]), "b2": f32(sd[p + "ffn.output_proj.bias"]),
-                "ffn_ln_g": f32(sd[p + "ffn_layer_norm.weight"]), "ffn_ln_b": f32(sd[p + "ffn_layer_norm.bias"]),
-            })
         fw = torch.zeros((d, 192), dtype=torch.float32)
         fw[:, : config.feature_dim] = sd["encoder_frontend.model_dim_proj.weight"].float()
-        # TransformerEmbeddingFrontend(embed, SinusoidalPositionEncoder): E[bos] * sqrt(d) + pos[0] = [0.. | 1..]  [fs2]
-        q0 = sd["encoder_pooler.decoder_frontend.embed.weight"][config.bos_idx].float() * math.sqrt(d)
-        q0 = q0 + torch.cat([torch.zeros(d // 2), torch.ones(d // 2)])
-        top = {
+        top, pooler = self._pooler_weights(sd, "encoder_pooler", config.bos_idx, d)  # projection_out has no bias
+        top.update({
             "front_ln_g": f32(sd["encoder_frontend.post_extract_layer_norm.weight"]),
             "front_ln_b": f32(sd["encoder_frontend.post_extract_layer_norm.bias"]),
             "front_w": bf(fw), "front_b": f32(sd["encoder_frontend.model_dim_proj.bias"]),
             "final_ln_g": f32(sd["layer_norm.weight"]), "final_ln_b": f32(sd["layer_norm.bias"]),
-            "pooler_q0": f32(q0), "proj_w": bf(sd["encoder_pooler.projection_out.weight"]),
             "zeros": f32(torch.zeros(8192)),
-        }
+        })
         w_c = _lib.SbSpeechWeights(layers=self._layer_array(_lib.SbConformerLayerWeights, layers),
                                    pooler=self._layer_array(_lib.SbPoolerLayerWeights, pooler),
                                    **{k: v.data_ptr() for k, v in top.items()})

@@ -207,7 +207,10 @@ class B200TextEncoderModel(EngineModel):
             })
 
         attn = self.pooling == Pooling.ATTENTION
-        pooler_layers = self._pooler_weights(sd, top) if attn else []
+        pooler_layers = []
+        if attn:
+            pooler_top, pooler_layers = self._pooler_weights(sd, "pooler", 0, self.embedding_dim)
+            top.update(pooler_top)
         cfg_c = _lib.SbEncoderConfig(
             model_dim=d, num_layers=L, num_heads=config.num_encoder_attn_heads, ffn_inner_dim=config.ffn_inner_dim,
             vocab_size=config.vocab_info.size, pos_rows=max_len, pooling=self.pooling.value, ln_eps=1e-5,
@@ -222,37 +225,6 @@ class B200TextEncoderModel(EngineModel):
             w_c.pooler = self._layer_array(_lib.SbPoolerLayerWeights, pooler_layers)
         self._create(cfg_c, w_c)
         self.return_encoded_seqs = False
-
-    def _pooler_weights(self, sd: Dict[str, Tensor], top: Dict[str, Tensor]) -> List[Dict[str, Tensor]]:
-        """The attention pooler's tensors in the engine's layout (``SbEncoderWeights.pooler_q0 / proj_w / proj_b``
-        added to ``top``; one ``SbPoolerLayerWeights`` dict per decoder layer)."""
-        e = self.embedding_dim
-        bf, f32 = self._bf16, self._f32
-        # the single decoder input: TransformerEmbeddingFrontend of token bos_idx = 0 = embed[0] * sqrt(E) + the
-        # sinusoid of position 0, [sin 0 ... | cos 0 ...] = [0 ... | 1 ...]  [fs2]
-        pos0 = torch.cat([torch.zeros(e // 2), torch.ones(e - e // 2)])
-        top["pooler_q0"] = f32(sd["pooler.decoder_frontend.embed.weight"][0].float() * math.sqrt(e) + pos0)
-        top["proj_w"] = bf(sd["pooler.projection_out.weight"])
-        top["proj_b"] = f32(sd["pooler.projection_out.bias"])
-        layers = []
-        for i in range(self.config.num_decoder_layers):
-            p = f"pooler.decoder.layers.{i}."
-            sa, ca = p + "self_attn.", p + "encoder_decoder_attn."
-            layers.append({
-                "sa_wv": bf(sd[sa + "v_proj.weight"]), "sa_bv": f32(sd[sa + "v_proj.bias"]),
-                "sa_wo": bf(sd[sa + "output_proj.weight"]), "sa_bo": f32(sd[sa + "output_proj.bias"]),
-                "sa_ln_g": f32(sd[p + "self_attn_layer_norm.weight"]), "sa_ln_b": f32(sd[p + "self_attn_layer_norm.bias"]),
-                "ca_wq": bf(sd[ca + "q_proj.weight"]), "ca_bq": f32(sd[ca + "q_proj.bias"]),
-                "ca_wkv": bf(torch.cat([sd[ca + "k_proj.weight"], sd[ca + "v_proj.weight"]], 0)),
-                "ca_bkv": f32(torch.cat([sd[ca + "k_proj.bias"], sd[ca + "v_proj.bias"]], 0)),
-                "ca_wo": bf(sd[ca + "output_proj.weight"]), "ca_bo": f32(sd[ca + "output_proj.bias"]),
-                "ca_ln_g": f32(sd[p + "encoder_decoder_attn_layer_norm.weight"]),
-                "ca_ln_b": f32(sd[p + "encoder_decoder_attn_layer_norm.bias"]),
-                "w1": bf(sd[p + "ffn.inner_proj.weight"]), "b1": f32(sd[p + "ffn.inner_proj.bias"]),
-                "w2": bf(sd[p + "ffn.output_proj.weight"]), "b2": f32(sd[p + "ffn.output_proj.bias"]),
-                "ffn_ln_g": f32(sd[p + "ffn_layer_norm.weight"]), "ffn_ln_b": f32(sd[p + "ffn_layer_norm.bias"]),
-            })
-        return layers
 
     @torch.inference_mode()
     def forward(self, batch: SequenceBatch) -> SonarEncoderOutput:

@@ -45,15 +45,19 @@ def test_fbank_rejects_bad_input(native_lib, cuda_device):
 
 
 # ---------------------------------------------------------------- Conformer encoder + pooler vs the oracle
-@pytest.fixture(scope="module")
-def speech_small(native_lib, cuda_device):
+def _speech_models(pooler_layers, device):
     from oracle.speech_encoder import OracleSpeechConfig, OracleSpeechEncoder, make_synthetic_speech_state_dict
     from sonar_b200 import B200SpeechEncoderModel, sonar_speech_encoder_config
 
-    ocfg = OracleSpeechConfig(num_layers=2, pooler_layers=2)
+    ocfg = OracleSpeechConfig(num_layers=2, pooler_layers=pooler_layers)
     sd = make_synthetic_speech_state_dict(ocfg, seed=3)
-    cfg = sonar_speech_encoder_config("english", num_encoder_layers=2, num_decoder_layers=2)
-    return OracleSpeechEncoder(ocfg, sd), B200SpeechEncoderModel(cfg, sd, cuda_device)  # default attention kernel (mma.sync)
+    cfg = sonar_speech_encoder_config("english", num_encoder_layers=2, num_decoder_layers=pooler_layers)
+    return OracleSpeechEncoder(ocfg, sd), B200SpeechEncoderModel(cfg, sd, device)  # default attention kernel (mma.sync)
+
+
+@pytest.fixture(scope="module")
+def speech_small(native_lib, cuda_device):
+    return _speech_models(2, cuda_device)
 
 
 def _speech_check(m, what):
@@ -65,26 +69,27 @@ def test_speech_encoder_vs_oracle(speech_small, cuda_device):
     from sonar_b200 import PaddingMask, SequenceBatch
     from tests.helpers import parity_metrics
 
-    oracle, model = speech_small
     g = torch.Generator().manual_seed(5)
     frames = [300, 131, 64, 257, 2]
     tmax = 300
     fb = torch.zeros((len(frames), tmax, 80))
     for i, n in enumerate(frames):
         fb[i, :n] = torch.randn((n, 80), generator=g)
-    ref, ref_enc, lens = oracle(fb, frames)
-    model.return_encoded_seqs = True
-    out = model(SequenceBatch(fb.to(cuda_device), PaddingMask(torch.tensor(frames), tmax, frames)))
-    model.return_encoded_seqs = False
-    torch.cuda.synchronize()
-    # encoder states (after model.layer_norm) at the real positions, packed order
-    start = 0
-    for i, n in enumerate(lens):
-        got, exp = out.encoded_seqs[start : start + n].cpu(), ref_enc[i, :n]
-        rel = float((got - exp).norm() / exp.norm())
-        assert rel <= 2e-2, (i, rel)
-        start += n
-    _speech_check(parity_metrics(out.sentence_embeddings, ref), "speech 2+2 layers ragged")
+    for pooler_layers in (2, 6):  # the fixture's pooler, and the `non_english` pooler depth
+        oracle, model = speech_small if pooler_layers == 2 else _speech_models(pooler_layers, cuda_device)
+        ref, ref_enc, lens = oracle(fb, frames)
+        model.return_encoded_seqs = True
+        out = model(SequenceBatch(fb.to(cuda_device), PaddingMask(torch.tensor(frames), tmax, frames)))
+        model.return_encoded_seqs = False
+        torch.cuda.synchronize()
+        # encoder states (after model.layer_norm) at the real positions, packed order
+        start = 0
+        for i, n in enumerate(lens):
+            got, exp = out.encoded_seqs[start : start + n].cpu(), ref_enc[i, :n]
+            rel = float((got - exp).norm() / exp.norm())
+            assert rel <= 2e-2, (pooler_layers, i, rel)
+            start += n
+        _speech_check(parity_metrics(out.sentence_embeddings, ref), f"speech 2+{pooler_layers} layers ragged")
 
 
 def test_speech_batch_invariance_and_long_utterance(speech_small, cuda_device):
