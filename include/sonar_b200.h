@@ -432,6 +432,72 @@ int sb_beam_step(const float* lp, const int32_t* tok, const float* eos_lp, int64
                  int32_t eos_block, int32_t max_gen, int64_t vocab, int32_t eos, int32_t unk, int32_t pad,
                  float unk_penalty, float score_div, int32_t normalize, void* stream);
 
+/* ---- LASER2 text encoder: embedding + bidirectional multi-layer LSTM + max over time ----
+ * Replaces LaserLstmEncoder.forward(seqs, seq_lens) (sonar/nn/laser_lstm_encoder.py:60-116) built from the `laser2` config
+ * (sonar/models/laser2_text/config.py:28-38); parameter names are the module's own (embed_tokens.weight,
+ * lstm.{weight_ih,weight_hh,bias_ih,bias_hh}_l{k}[_reverse]), with no converter (sonar/models/laser2_text/handler.py). */
+typedef struct SbLaser2 SbLaser2;
+
+typedef struct SbLaser2Config {
+  int64_t vocab_size;    /* 50004 */
+  int64_t pad_idx;       /* 1: positions holding this id are left out of the max (-inf) */
+  int32_t embed_dim;     /* 320 (model_dim; a positive multiple of 64) */
+  int32_t hidden_size;   /* 512 (the only supported value) */
+  int32_t num_layers;    /* 5 (>= 1) */
+  int32_t bidirectional; /* 1 (0 or 1) */
+  float padding_value;   /* 0.0: the value positions t >= len_b contribute to the max unless their id is pad_idx */
+  int32_t num_sms;       /* 0 = query the device */
+} SbLaser2Config;
+
+/* One torch.nn.LSTM layer and direction; DEVICE pointers, caller-owned, gate order i, f, g, o. */
+typedef struct SbLstmLayerWeights {
+  const void* w_ih;   /* bf16 [4H, in]  weight_ih_l{k}[_reverse]; in = embed_dim for k = 0, else H * (1 + bidirectional) */
+  const void* w_hh;   /* bf16 [4H, H]   weight_hh_l{k}[_reverse] */
+  const float* b_ih;  /* [4H] */
+  const float* b_hh;  /* [4H] */
+} SbLstmLayerWeights;
+
+typedef struct SbLaser2Weights {
+  const void* embed;                /* bf16 [vocab, embed_dim]  embed_tokens.weight */
+  const SbLstmLayerWeights* layers; /* HOST array of num_layers * (1 + bidirectional) entries: entry k * dirs + d is layer k,
+                                     * direction d (d = 1: the _reverse weights); copied at create */
+} SbLaser2Weights;
+
+/* Allocates the handle's own device memory (a 256-byte input-check flag and the weights repacked into the recurrent kernel's
+ * gate order with b_ih + b_hh summed: 57 MB for `laser2`; the caller's weights are not modified) and a pinned host staging
+ * ring, and synchronises the device once.  Fails with SB_ERR_CUDA when one 16-CTA cluster of the recurrent kernel does not
+ * fit on the device. */
+int sb_laser2_create(const SbLaser2Config* cfg, const SbLaser2Weights* w, SbLaser2** out);
+void sb_laser2_destroy(SbLaser2* enc);
+/* Bytes of device workspace for <= max_batch sequences holding <= max_tokens real tokens in total. */
+int sb_laser2_workspace_bytes(const SbLaser2* enc, int32_t max_batch, int64_t max_tokens, size_t* bytes);
+/* ids            DEVICE int64 [batch, ids_row_stride >= seq_len], right-padded with any value
+ * seq_lens_host  HOST int32 [batch] lengths in 1..seq_len (NULL = all seq_len); a zero length is SB_ERR_INVALID, as
+ *                pack_padded_sequence refuses it
+ * out            DEVICE fp32 [batch, H * (1 + bidirectional)] = max over t < seq_len of the [fwd | bwd] outputs, where a
+ *                position t >= len_b contributes padding_value and a position whose id is pad_idx contributes -inf
+ * batch <= 32768.  Asynchronous on `stream`; never allocates. */
+int sb_laser2_forward(SbLaser2* enc, const int64_t* ids, int64_t ids_row_stride, const int32_t* seq_lens_host, int32_t batch,
+                      int32_t seq_len, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* Checks the sticky device-side flag (token id outside [0, vocab_size)) of the forwards since the last check; synchronises
+ * `stream`.  Returns SB_OK or SB_ERR_INPUT. */
+int sb_laser2_check_inputs(SbLaser2* enc, void* stream);
+
+/* The LSTM recurrence alone (H = 512), for one layer and `num_dirs` directions.  Gate order: row / column
+ * d * 4H + 128 c + 32 gate + u of the operands below is gate `gate` (i, f, g, o) of hidden unit 32 c + u of direction d.
+ *   G          DEVICE bf16 [T, ldg >= num_dirs * 4H] input pre-activations X . W_ih^T + b_ih + b_hh of the packed tokens
+ *   w_hh       DEVICE bf16 [num_dirs * 4H, H] in the gate order above
+ *   cu_seqlens DEVICE int32 [B + 1]: the tokens of sequence b are rows cu[b] .. cu[b + 1] - 1
+ *   tile_seqs  DEVICE int32 [num_tiles * 64]: the sequences of each 64-row tile, -1 = empty row
+ * and exactly one of
+ *   y          DEVICE bf16 [T, ldy]: h_t of direction d at columns d * H (the reverse direction runs from the last token)
+ *   pool_out   DEVICE fp32 [B, ldp]: max over the sequence's tokens of h_t, skipping tokens with pad_mask[token] != 0
+ *              (DEVICE uint8 [T] or NULL), then max with padding_value where tail_keep[b] != 0 (DEVICE uint8 [B] or NULL);
+ *              only sequences named in tile_seqs are written. */
+int sb_lstm_recurrent(const void* G, int64_t ldg, const void* w_hh, const int32_t* cu_seqlens, const int32_t* tile_seqs,
+                      int32_t num_tiles, int32_t num_dirs, void* y, int64_t ldy, float* pool_out, int64_t ldp,
+                      const uint8_t* pad_mask, const uint8_t* tail_keep, float padding_value, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -85,6 +85,20 @@ class SbSpeechWeights(C.Structure):
                [("layers", C.POINTER(SbConformerLayerWeights)), ("pooler", C.POINTER(SbPoolerLayerWeights))]
 
 
+class SbLaser2Config(C.Structure):
+    _fields_ = [("vocab_size", C.c_int64), ("pad_idx", C.c_int64), ("embed_dim", C.c_int32), ("hidden_size", C.c_int32),
+                ("num_layers", C.c_int32), ("bidirectional", C.c_int32), ("padding_value", C.c_float),
+                ("num_sms", C.c_int32)]
+
+
+class SbLstmLayerWeights(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("w_ih", "w_hh", "b_ih", "b_hh")]
+
+
+class SbLaser2Weights(C.Structure):
+    _fields_ = [("embed", C.c_void_p), ("layers", C.POINTER(SbLstmLayerWeights))]
+
+
 # name -> (restype, argtypes); must list every symbol include/sonar_b200.h declares
 _SIGNATURES = {
     "sb_last_error": (C.c_char_p, []),
@@ -149,6 +163,15 @@ _SIGNATURES = {
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "sb_beam_step": (C.c_int, [C.c_void_p] * 13 + [C.c_int32] * 7 + [C.c_int64] + [C.c_int32] * 3 +
                      [C.c_float, C.c_float, C.c_int32, C.c_void_p]),
+    "sb_laser2_create": (C.c_int, [C.POINTER(SbLaser2Config), C.POINTER(SbLaser2Weights), C.POINTER(C.c_void_p)]),
+    "sb_laser2_destroy": (None, [C.c_void_p]),
+    "sb_laser2_workspace_bytes": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_size_t)]),
+    "sb_laser2_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                    C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sb_laser2_check_inputs": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "sb_lstm_recurrent": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                    C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float,
+                                    C.c_void_p]),
 }
 
 

@@ -191,3 +191,45 @@ def pool_latent_attention(qt: Tensor, mem: Tensor, cu_seqlens: Tensor) -> Tensor
                                               u.data_ptr(), _stream())
     _lib.check(rc, "sb_pool_latent_attention")
     return u
+
+
+LSTM_TILE_ROWS = 64  # sequences per tile of the LSTM recurrent kernel
+
+
+def lstm_gate_rows(hidden_size: int = 512, num_dirs: int = 1) -> Tensor:
+    """int64 [num_dirs * 4H]: entry n is the row of torch.nn.LSTM's stacked [i | f | g | o] gate matrices (of direction
+    n // 4H) that row n of the LSTM kernels' gate order holds: row 128 c + 32 gate + u is gate `gate` of hidden unit
+    32 c + u, so each 16th of the hidden units has its four gates together."""
+    n = torch.arange(4 * hidden_size)
+    one = (n % 128) // 32 * hidden_size + n // 128 * 32 + n % 32
+    return torch.cat([one + d * 4 * hidden_size for d in range(num_dirs)])
+
+
+def lstm_recurrent(g: Tensor, w_hh: Tensor, cu_seqlens: Tensor, tile_seqs: Tensor, num_dirs: int, *,
+                   pool: bool = False, pad_mask: Optional[Tensor] = None, tail_keep: Optional[Tensor] = None,
+                   padding_value: float = 0.0) -> Tensor:
+    """The LSTM recurrence (H = 512) of one layer on packed tokens, everything in ``lstm_gate_rows`` order:
+    g bf16 [T, num_dirs * 4H] input pre-activations (x . W_ih^T + b_ih + b_hh), w_hh bf16 [num_dirs * 4H, H],
+    cu_seqlens int32 [B + 1], tile_seqs int32 [tiles * 64] (sequence per tile row, -1 = empty).  Returns the outputs
+    bf16 [T, num_dirs * H], or with ``pool`` fp32 [B, num_dirs * H]: the max over each sequence's tokens, skipping those
+    with pad_mask (uint8 [T]) set, then max with ``padding_value`` where tail_keep (uint8 [B]) is set; rows of sequences
+    missing from tile_seqs are left uninitialised."""
+    _need_cuda(g, w_hh, cu_seqlens, tile_seqs, pad_mask, tail_keep)
+    assert g.dtype == torch.bfloat16 and w_hh.dtype == torch.bfloat16 and g.stride(1) == 1 and w_hh.is_contiguous()
+    assert cu_seqlens.dtype == torch.int32 and tile_seqs.dtype == torch.int32 and tile_seqs.numel() % LSTM_TILE_ROWS == 0
+    h = w_hh.shape[1]
+    assert w_hh.shape[0] == num_dirs * 4 * h and g.shape[1] >= num_dirs * 4 * h
+    for m in (pad_mask, tail_keep):
+        assert m is None or m.dtype == torch.uint8
+    t, b = g.shape[0], cu_seqlens.numel() - 1
+    if pool:
+        out = torch.empty((b, num_dirs * h), dtype=torch.float32, device=g.device)
+        y, pool_out, ld = None, out, out.stride(0)
+    else:
+        out = torch.empty((t, num_dirs * h), dtype=torch.bfloat16, device=g.device)
+        y, pool_out, ld = out, None, out.stride(0)
+    rc = _lib.load().sb_lstm_recurrent(g.data_ptr(), g.stride(0), w_hh.data_ptr(), cu_seqlens.data_ptr(), tile_seqs.data_ptr(),
+                                       tile_seqs.numel() // LSTM_TILE_ROWS, num_dirs, _ptr(y), ld, _ptr(pool_out), ld,
+                                       _ptr(pad_mask), _ptr(tail_keep), padding_value, _stream())
+    _lib.check(rc, "sb_lstm_recurrent")
+    return out

@@ -7,6 +7,7 @@
   ``__lang__`` control symbols; source encoding ``[__lang__] + pieces + [</s>]``;
   SURVEY App. F1).  Needs the ``sentencepiece.bpe.model`` file, which is not available
   offline; the class exists so real checkpoints work wherever the files do.
+* ``Laser2Tokenizer`` wraps the LASER2 SentencePiece model (``laser2.spm``; tokenizer family ``lstm``).
 * ``SyntheticTokenizer`` is a dependency-free stand-in (hashes whitespace words into the
   piece id range) for tests and benchmarks: same control-token layout, deterministic.
 """
@@ -126,3 +127,32 @@ class NllbTokenizer:
             return sp.decode([i - 1 for i in ids if 4 <= i <= n])
 
         return _TokenDecoder(dec)
+
+
+class Laser2Tokenizer:
+    """The LASER2 tokenizer (``sonar/models/laser2_text/tokenizer.py:27-87``): SentencePiece ids with a ``</s>`` suffix,
+    then ``id + 4`` for every id >= 3, so ids 0 (``<unk>``) and 2 (``</s>``) are unchanged and 1 is never produced.
+    Batches are padded with ``vocab_info.pad_idx`` = 1, the id the ``laser2`` config masks (``config.py:33``).
+
+    The reference builds its vocabulary information through fairseq2's ``SentencePieceModel(path, ["<pad>"])`` and
+    ``vocab_info_from_sentencepiece`` [fs2]; which id fairseq2 gives the added ``<pad>`` control symbol is not pinned
+    here.  ``pad_idx`` = 1 is what the model and the reference's own test (``Collater(pad_value=1)``) use."""
+
+    def __init__(self, spm_path: str) -> None:
+        import sentencepiece as spm  # local import: optional dependency
+
+        self._sp = spm.SentencePieceProcessor(model_file=str(spm_path))
+        # shifted piece ids reach piece_size + 3
+        self.vocab_info = VocabularyInfo(size=self._sp.get_piece_size() + 4, unk_idx=0, bos_idx=None, eos_idx=2, pad_idx=1)
+
+    def create_encoder(self, *, task: Optional[str] = None, lang: Optional[str] = None, mode: Optional[str] = None,
+                       device=None, pin_memory: bool = False) -> _TokenEncoder:
+        """No language: LASER2 is language-agnostic.  ``task`` / ``lang`` / ``mode`` are accepted and ignored, as in the
+        reference."""
+        sp = self._sp
+        eos = sp.eos_id()
+
+        def enc(text: str) -> List[int]:
+            return [i + 4 if i >= 3 else i for i in sp.encode(text) + [eos]]
+
+        return _TokenEncoder(enc, suffix=[eos])
