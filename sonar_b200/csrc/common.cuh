@@ -213,6 +213,18 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// Four 8x8 b16 matrices from the mma fragment layout (lane l holds row l / 4, columns 2 (l % 4), + 1 of matrix i in
+// r[i]) to shared memory; lanes 8 i .. 8 i + 7 give the addresses of the eight 16-byte rows of matrix i.
+__device__ __forceinline__ void stmatrix_x4(uint32_t smem_addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+
+__device__ __forceinline__ void st_shared_v2(uint32_t smem_addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_addr), "f"(x), "f"(y) : "memory");
+}
+
 // ----------------------------------------------------------------------------
 // wgmma (Hopper warpgroup MMA): bf16 x bf16 -> fp32 accumulators in registers
 // ----------------------------------------------------------------------------

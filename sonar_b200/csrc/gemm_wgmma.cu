@@ -12,10 +12,13 @@
 //   per pair.  cta_group = 1: independent CTAs.
 // Warp roles (384 threads): warpgroup 0 = producer (one thread issues TMA; the group gives its registers away with
 //   setmaxnreg), warpgroups 1-2 = MMA + epilogue.
-// Epilogue: the accumulator fragments of 2 x 32 columns at a time go through a padded shared-memory buffer so that ONE
-//   THREAD OWNS ONE ROW of 32 consecutive columns (thread t of the warpgroup: row t % 64, column half t / 64 of the
-//   tile) -- the layout the row-wise epilogues (LayerNorm statistics, running top-k, log-sum-exp) are written for --
-//   then bias/ReLU/residual -> swizzled smem -> TMA store.
+// Epilogue, column-wise modes (bias, ReLU, SiLU, residual, accumulate, LnFold consumer): every thread applies bias and
+//   activation to its accumulator fragments in registers and writes them straight into the 128B-swizzled staging
+//   layout of the TMA store (stmatrix for bf16, st.shared.v2 for fp32), one 64-row x 128-byte box at a time, double
+//   buffered, so the store of one box reads while the next is written.
+// Epilogue, row-wise modes (LayerNorm statistics, running top-k / log-sum-exp): the fragments of 2 x 32 columns at a
+//   time go through a padded shared-memory buffer so that ONE THREAD OWNS ONE ROW of 32 consecutive columns (thread t
+//   of the warpgroup: row t % 64, column half t / 64 of the tile), then swizzled smem -> TMA store.
 // LayerNorm folding (LnFold, sonar_b200_internal.h): a consumer GEMM scales its accumulator rows by the LayerNorm
 // statistics of its input; the residual-stream GEMMs emit those statistics and the bf16 copy of the stream.
 // Operand smem layout: K-major, 128-byte rows, SWIZZLE_128B (TMA writes it, wgmma reads it).
@@ -27,24 +30,36 @@
 
 namespace sb {
 
-template <int kCtaGroup>
+// The row-wise epilogues need one thread per row (the fragment -> row transposition buffer); the others are column-wise.
+constexpr bool epi_row_wise(int epi) { return epi == EPI_BIAS_RESIDUAL_STATS || epi == EPI_TOPK; }
+
+// Shared memory: the row-wise epilogues keep 3 ring stages next to their transposition buffers (2 x 17 KB); the
+// column-wise ones have no such buffer and spend the space on a 4th stage, so the producer can run 4 k-blocks of the next
+// tile ahead while the epilogue runs.  The other layout that fits, 3 stages and four staging boxes per warpgroup (a whole
+// bf16 tile, one store wait per tile), measured slower in the same run on an H100 SXM (700 W): 3.35 k against 3.39 k
+// sentences/s in bench.py, FFN1 alone 469 against 473 TFLOP/s, FFN2 510 against 523.
+template <int kCtaGroup, int kEpi>
 struct GemmCfg {
+  static constexpr bool ROW_WISE = epi_row_wise(kEpi);
   static constexpr int BLOCK_M = 128;                 // rows per CTA (64 per consumer warpgroup)
   static constexpr int BLOCK_N = 256;                 // wgmma N
   static constexpr int BLOCK_K = 64;                  // 128 bytes of bf16 = one swizzle atom
   static constexpr int LOAD_N = BLOCK_N / kCtaGroup;  // W rows each CTA loads (multicast to the pair)
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
   static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
-  static constexpr int STAGES = 3;                    // 48 KB per mainloop stage
+  static constexpr int STAGES = ROW_WISE ? 3 : 4;     // 48 KB per mainloop stage
   static constexpr int EPI_GROUPS = 2;                // column halves of a tile row = row-wise result lists per tile
-  static constexpr int CD_BYTES = 2 * 64 * 128;       // per consumer warpgroup: 64 rows x 128 B for each column half
+  static constexpr int CD_BYTES = 2 * 64 * 128;       // per consumer warpgroup: two 64-row x 128-byte TMA boxes
   static constexpr int TRANS_LD = 68;                 // floats per row of the fragment -> row-per-thread buffer (64 + pad)
-  static constexpr int TRANS_BYTES = 64 * TRANS_LD * 4;
+  static constexpr int TRANS_BYTES = ROW_WISE ? 64 * TRANS_LD * 4 : 0;
+  static constexpr int LN_BYTES = 64 * 8;             // per consumer warpgroup: (mean, rstd) of its rows (LnFold consumer)
   static constexpr int BAR_BYTES = 256;
-  static constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 2 * (CD_BYTES + TRANS_BYTES) + BAR_BYTES + 1024 /*align slack*/;
+  static constexpr int SMEM_BYTES =
+      STAGES * (A_BYTES + B_BYTES) + 2 * (CD_BYTES + TRANS_BYTES + LN_BYTES) + BAR_BYTES + 1024 /*align slack*/;
   static constexpr int THREADS = 384;
+  static_assert(SMEM_BYTES <= 232448, "shared memory budget of one sm_90 block");
+  static_assert(2 * STAGES * 8 <= BAR_BYTES, "ring barriers");
 };
-static_assert(GemmCfg<1>::SMEM_BYTES <= 232448, "shared memory budget of one sm_90 block");
 
 // Tile scheduler shared by the three warp roles (each role walks an identical copy).
 // Default: tiles are dealt round-robin with n fastest, so the clusters running concurrently share A rows
@@ -111,21 +126,22 @@ __device__ __forceinline__ void topk_insert(float (&tv)[KC], int (&ti)[KC], floa
 
 
 template <int kCtaGroup, int kEpi, typename OutT>
-__global__ void __launch_bounds__(GemmCfg<kCtaGroup>::THREADS, 1)
+__global__ void __launch_bounds__(GemmCfg<kCtaGroup, kEpi>::THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                        const __grid_constant__ CUtensorMap tm_c, const float* __restrict__ bias,
                        const OutT* residual, long long ldr, int M, int N, int K, float* __restrict__ cand_val,
                        int* __restrict__ cand_idx, float* __restrict__ lse_part, int n_chunks, const LnFold lf,
                        const ColFilter cf, int k_splits, int* __restrict__ splitk_flags) {
   constexpr bool kSweep = (kEpi == EPI_TOPK);
-  using Cfg = GemmCfg<kCtaGroup>;
+  using Cfg = GemmCfg<kCtaGroup, kEpi>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem_a + Cfg::STAGES * Cfg::A_BYTES;
   uint8_t* smem_cd = smem_b + Cfg::STAGES * Cfg::B_BYTES;
   uint8_t* smem_tr = smem_cd + 2 * Cfg::CD_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_tr + 2 * Cfg::TRANS_BYTES);
+  uint8_t* smem_ln = smem_tr + 2 * Cfg::TRANS_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_ln + 2 * Cfg::LN_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
 
   const int warp_idx = threadIdx.x >> 5;
@@ -190,10 +206,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
     const int erow = t & 63;              // ... of row erow of this warpgroup
     const int row_in_tile = cwg * 64 + erow;
     const int frow = (warp_idx & 3) * 16 + (lane >> 2);  // accumulator fragment: rows frow and frow + 8
-    constexpr int CHUNK_COLS = 128 / int(sizeof(OutT));  // one 128-byte smem row per output row
-    constexpr int SUBS = CHUNK_COLS / 32;                // 32-column pieces per staged chunk
     uint8_t* smem_cd_wg = smem_cd + cwg * Cfg::CD_BYTES;
     float* trans = reinterpret_cast<float*>(smem_tr + cwg * Cfg::TRANS_BYTES);
+    float2* ln_sm = reinterpret_cast<float2*>(smem_ln + cwg * Cfg::LN_BYTES);
     const uint32_t bar_id = 1 + cwg;  // named barrier of this warpgroup
     const uint64_t a_desc0 = wgmma_desc_kmajor_sw128(smem_u32(smem_a) + cwg * 64 * 128);
     const uint64_t b_desc0 = wgmma_desc_kmajor_sw128(smem_u32(smem_b));
@@ -249,6 +264,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
               if (i < lf.chunks) { const float dm = part_next[i].x - ln_mean; m2 += part_next[i].y + float(kLnPartCols) * dm * dm; }
             ln_rstd = 1.0f / sqrtf(m2 / float(kLnPartCols * lf.chunks) + lf.eps);
           }
+          // to the fragment layout (read after the mainloop; the previous tile read its values before its last store)
+          if (half == 0) ln_sm[erow] = make_float2(ln_mean, ln_rstd);
           fetch_parts();  // for the next tile
         }
       }
@@ -294,6 +311,111 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
         release(prev);
+      }
+      if constexpr (!Cfg::ROW_WISE) {
+        // ---- column-wise epilogue from the accumulator fragments: rows frow and frow + 8, columns 8 j + 2 (lane % 4), + 1 ----
+        // Box b = the warpgroup's 64 rows x columns [b * BOX_COLS, (b + 1) * BOX_COLS) of the tile, 128 bytes per row, in
+        // the 128B-swizzled layout of the TMA store (16-byte chunk q of row r at q ^ (r % 8)).  Boxes alternate between
+        // two staging buffers: before the barrier that publishes box b, thread 0 waits until the store of box b - 1 has
+        // read its buffer, which box b + 1 is written into.
+        constexpr int BOX_COLS = 128 / int(sizeof(OutT));
+        constexpr int BOXES = Cfg::BLOCK_N / BOX_COLS;
+        constexpr int BOX_BYTES = 64 * 128;
+        constexpr int NBUF = Cfg::CD_BYTES / BOX_BYTES;
+        static_assert(NBUF >= 2 && BOXES % NBUF == 0, "staging buffers must alternate the same way in every tile");
+        const int fcol = 2 * (lane & 3);                     // first of this thread's two columns in each 8-column group
+        const int grow_lo = m0 + cwg * 64 + frow, grow_hi = grow_lo + 8;
+        if (fold_in) named_bar_sync(bar_id, 128);  // ln_sm of this tile is complete
+        // split-K: the bias belongs to split 0, the later splits add their bare partial products
+        const bool with_bias = !(kEpi == EPI_BIAS_ACCUM && chunk > 0);
+        // fl(acc + bias) or the LnFold rstd * (acc - mean * c) + b', then the activation or the residual add
+        auto epi = [&](float v, float b, float c, float2 ln, int grow, int col) -> float {
+          float f = fold_in ? fmaf(ln.y, fmaf(-ln.x, c, v), b) : v + b;
+          if constexpr (kEpi == EPI_BIAS_RELU) f = fmaxf(f, 0.0f);
+          if constexpr (kEpi == EPI_BIAS_SILU) f = silu_fast(f);
+          if constexpr (kEpi == EPI_BIAS_RESIDUAL) {
+            if (grow < M) {
+              if constexpr (sizeof(OutT) == 4) f += reinterpret_cast<const float*>(residual)[(long long)grow * ldr + col];
+              else f += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(residual)[(long long)grow * ldr + col]);
+            }
+          }
+          return f;
+        };
+        // the 8-column group j of the tile: bias (and LnFold colsum) of this thread's two columns, then both rows
+        auto group = [&](int j, float (&o)[4]) {
+          const int col = n0 + 8 * j + fcol;
+          const float2 b2 = with_bias ? __ldg(reinterpret_cast<const float2*>(bias + col)) : make_float2(0.f, 0.f);
+          const float2 c2 = fold_in ? __ldg(reinterpret_cast<const float2*>(lf.colsum + col)) : make_float2(0.f, 0.f);
+          // (mean, rstd) of rows frow, frow + 8, read where they are used: not held in registers across the epilogue
+          const float2 ln_lo = fold_in ? ln_sm[frow] : make_float2(0.f, 1.f);
+          const float2 ln_hi = fold_in ? ln_sm[frow + 8] : make_float2(0.f, 1.f);
+          o[0] = epi(acc[4 * j + 0], b2.x, c2.x, ln_lo, grow_lo, col);
+          o[1] = epi(acc[4 * j + 1], b2.y, c2.y, ln_lo, grow_lo, col + 1);
+          o[2] = epi(acc[4 * j + 2], b2.x, c2.x, ln_hi, grow_hi, col);
+          o[3] = epi(acc[4 * j + 3], b2.y, c2.y, ln_hi, grow_hi, col + 1);
+        };
+        const uint32_t cd_base = smem_u32(smem_cd_wg);
+#pragma unroll
+        for (int b = 0; b < BOXES; ++b) {
+          const uint32_t buf = cd_base + (b % NBUF) * BOX_BYTES;
+          if constexpr (sizeof(OutT) == 2) {
+            // stmatrix x4 per 16 columns: matrices (rows 0-7, j), (rows 8-15, j), (rows 0-7, j + 1), (rows 8-15, j + 1)
+            // of the warp's 16 rows; lane l addresses row l % 8 of matrix l / 8
+            const int mrow = (warp_idx & 3) * 16 + (lane & 7) + 8 * ((lane >> 3) & 1);
+#pragma unroll
+            for (int p = 0; p < BOX_COLS / 16; ++p) {
+              const int j = b * (BOX_COLS / 8) + 2 * p;
+              float o0[4], o1[4];
+              group(j, o0);
+              group(j + 1, o1);
+              const int q = 2 * p + (lane >> 4);
+              stmatrix_x4(buf + mrow * 128 + ((q ^ (lane & 7)) << 4), pack_bf16x2(o0[0], o0[1]), pack_bf16x2(o0[2], o0[3]),
+                          pack_bf16x2(o1[0], o1[1]), pack_bf16x2(o1[2], o1[3]));
+            }
+          } else {
+            // 8 bytes per row and group: byte 4 fcol of the group's 32 bytes
+#pragma unroll
+            for (int jj = 0; jj < BOX_COLS / 8; ++jj) {
+              float o[4];
+              group(b * (BOX_COLS / 8) + jj, o);
+              const int q = 2 * jj + ((lane >> 1) & 1);
+              const uint32_t a = buf + frow * 128 + ((q ^ (frow & 7)) << 4) + 8 * (lane & 1);
+              st_shared_v2(a, o[0], o[1]);
+              st_shared_v2(a + 8 * 128, o[2], o[3]);
+            }
+          }
+          fence_proxy_async_smem();
+          if (t == 0) tma_store_wait_read<NBUF - 2>();
+          named_bar_sync(bar_id, 128);
+          if (t == 0) {
+            const int c0 = n0 + b * BOX_COLS, r0 = m0 + cwg * 64;
+            if constexpr (kEpi == EPI_BIAS_ACCUM) {
+              // Ordered split-K: the splits of a tile add into C one after the other (x + p0, + p1, + p2 -- the same sum on
+              // every run).  Split s waits for the counter its predecessor leaves after ITS adds have completed; the
+              // predecessor is a lower-numbered item, so it is already running on another resident cluster or finished.
+              int* flag = nullptr;
+              if (k_splits > 1) {
+                flag = splitk_flags + ((long long)(m_blk * num_n_tiles + n_blk) * kCtaGroup + int(cta_rank)) * 2 + cwg;
+                if (b == 0 && chunk > 0) {
+                  while (ld_acquire_gpu(flag) != chunk) __nanosleep(64);
+                  fence_proxy_async_all();
+                }
+              }
+              tma_reduce_add_2d(&tm_c, reinterpret_cast<const void*>(smem_cd_wg + (b % NBUF) * BOX_BYTES), c0, r0);
+              tma_store_commit();
+              if (k_splits > 1 && b == BOXES - 1) {
+                tma_store_wait_all<0>();  // this split's adds have been performed
+                fence_proxy_async_all();
+                __threadfence();
+                st_release_gpu(flag, chunk == k_splits - 1 ? 0 : chunk + 1);  // the last split re-arms the counter
+              }
+            } else {
+              tma_store_2d(&tm_c, smem_cd_wg + (b % NBUF) * BOX_BYTES, c0, r0);
+              tma_store_commit();
+            }
+          }
+        }
+        continue;
       }
       // fragments of piece s (columns 32 s .. 32 s + 31 of both column halves) -> trans[row][half * 32 + column]
       auto stage_piece = [&](int s) {
@@ -432,40 +554,25 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
         }
         continue;
       }
+      // ---- residual + LayerNorm statistics (EPI_BIAS_RESIDUAL_STATS, fp32 C): one row of 32 columns per thread and piece ----
+      if constexpr (kEpi == EPI_BIAS_RESIDUAL_STATS) {
 #pragma unroll
-      for (int s = 0; s < 4; ++s) {
-        const int sub = s % SUBS;
-        if (sub == 0 && t == 0) tma_store_wait_read<0>();  // the staging buffer is free again (ordered by stage_piece's barrier)
-        uint32_t v[32];
-        stage_piece(s);
-        load_piece(v);
-        uint8_t* cd_row = smem_cd_wg + half * (64 * 128) + erow * 128;
-        const int col_in_tile = half * 128 + s * 32;
-        const int gcol = n0 + col_in_tile;
-        float f[32];
-        if (fold_in) {  // rstd * (x.W'^T - mean * c) + b'   (LnFold)
+        for (int s = 0; s < 4; ++s) {
+          if (t == 0) tma_store_wait_read<0>();  // the staging buffer is free again (ordered by stage_piece's barrier)
+          uint32_t v[32];
+          stage_piece(s);
+          load_piece(v);
+          uint8_t* cd_row = smem_cd_wg + half * (64 * 128) + erow * 128;
+          const int gcol = n0 + half * 128 + s * 32;
+          float f[32];
 #pragma unroll
           for (int j = 0; j < 32; j += 4) {
             const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + gcol + j));
-            const float4 c4 = __ldg(reinterpret_cast<const float4*>(lf.colsum + gcol + j));
-            f[j + 0] = fmaf(ln_rstd, fmaf(-ln_mean, c4.x, __uint_as_float(v[j + 0])), b4.x);
-            f[j + 1] = fmaf(ln_rstd, fmaf(-ln_mean, c4.y, __uint_as_float(v[j + 1])), b4.y);
-            f[j + 2] = fmaf(ln_rstd, fmaf(-ln_mean, c4.z, __uint_as_float(v[j + 2])), b4.z);
-            f[j + 3] = fmaf(ln_rstd, fmaf(-ln_mean, c4.w, __uint_as_float(v[j + 3])), b4.w);
-          }
-        } else {
-          // split-K: the bias belongs to split 0, the later splits add their bare partial products
-          const bool with_bias = !(kEpi == EPI_BIAS_ACCUM && chunk > 0);
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b4 = with_bias ? __ldg(reinterpret_cast<const float4*>(bias + gcol + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
             f[j + 0] = __uint_as_float(v[j + 0]) + b4.x;
             f[j + 1] = __uint_as_float(v[j + 1]) + b4.y;
             f[j + 2] = __uint_as_float(v[j + 2]) + b4.z;
             f[j + 3] = __uint_as_float(v[j + 3]) + b4.w;
           }
-        }
-        if constexpr (kEpi == EPI_BIAS_RESIDUAL_STATS) {
           // x_new = x + (acc + bias): the residual chunk was fetched one piece ahead; fetch the next one now
           float4 rcur[8];
 #pragma unroll
@@ -503,87 +610,19 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
               reinterpret_cast<float2*>(lf.stats_out)[((long long)grow * num_n_tiles + n_blk) * Cfg::EPI_GROUPS + half] =
                   make_float2(st_mean, st_m2);
           }
-        }
-        if constexpr (kEpi == EPI_BIAS_RELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.0f);
-        }
-        if constexpr (kEpi == EPI_BIAS_SILU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = silu_fast(f[j]);
-        }
-        if constexpr (kEpi == EPI_BIAS_RESIDUAL) {
-          if (grow < M) {
-            const OutT* rp = residual + (long long)grow * ldr + gcol;
-            if constexpr (sizeof(OutT) == 4) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 r4 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(rp) + j);
-                f[j + 0] += r4.x; f[j + 1] += r4.y; f[j + 2] += r4.z; f[j + 3] += r4.w;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {
-                const uint4 r8 = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(rp) + j);
-                const uint32_t w[4] = {r8.x, r8.y, r8.z, r8.w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const __nv_bfloat162 p = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
-                  f[j + 2 * q] += __low2float(p);
-                  f[j + 2 * q + 1] += __high2float(p);
-                }
-              }
-            }
-          }
-        }
-        // 128B-swizzled staging row: logical 16B chunk j lives at physical chunk j ^ (row % 8)
-        if constexpr (sizeof(OutT) == 4) {
+          // 128B-swizzled staging row: logical 16B chunk q lives at physical chunk q ^ (row % 8)
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             const int phys = q ^ (erow & 7);
-            *reinterpret_cast<float4*>(cd_row + phys * 16) =
-                make_float4(f[4 * q], f[4 * q + 1], f[4 * q + 2], f[4 * q + 3]);
+            *reinterpret_cast<float4*>(cd_row + phys * 16) = make_float4(f[4 * q], f[4 * q + 1], f[4 * q + 2], f[4 * q + 3]);
           }
-        } else {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int phys = (sub * 4 + q) ^ (erow & 7);
-            *reinterpret_cast<uint4*>(cd_row + phys * 16) =
-                make_uint4(pack_bf16x2(f[8 * q], f[8 * q + 1]), pack_bf16x2(f[8 * q + 2], f[8 * q + 3]),
-                           pack_bf16x2(f[8 * q + 4], f[8 * q + 5]), pack_bf16x2(f[8 * q + 6], f[8 * q + 7]));
-          }
-        }
-        if (sub == SUBS - 1) {  // both halves' [64 x 128 B] chunks are complete: two TMA stores
-          fence_proxy_async_smem();
+          fence_proxy_async_smem();  // both halves' [64 x 128 B] chunks are complete: two TMA stores
           named_bar_sync(bar_id, 128);
           if (t == 0) {
-            const int c0 = n0 + (s / SUBS) * CHUNK_COLS, r0 = m0 + cwg * 64;
-            if constexpr (kEpi == EPI_BIAS_ACCUM) {
-              // Ordered split-K: the splits of a tile add into C one after the other (x + p0, + p1, + p2 -- the same sum on
-              // every run).  Split s waits for the counter its predecessor leaves after ITS adds have completed; the
-              // predecessor is a lower-numbered item, so it is already running on another resident cluster or finished.
-              int* flag = nullptr;
-              if (k_splits > 1) {
-                flag = splitk_flags + ((long long)(m_blk * num_n_tiles + n_blk) * kCtaGroup + int(cta_rank)) * 2 + cwg;
-                if (s == 0 && chunk > 0) {
-                  while (ld_acquire_gpu(flag) != chunk) __nanosleep(64);
-                  fence_proxy_async_all();
-                }
-              }
-              tma_reduce_add_2d(&tm_c, smem_cd_wg, c0, r0);
-              tma_reduce_add_2d(&tm_c, smem_cd_wg + 64 * 128, c0 + 128, r0);
-              tma_store_commit();
-              if (k_splits > 1 && s == 3) {
-                tma_store_wait_all<0>();  // this split's adds have been performed
-                fence_proxy_async_all();
-                __threadfence();
-                st_release_gpu(flag, chunk == k_splits - 1 ? 0 : chunk + 1);  // the last split re-arms the counter
-              }
-            } else {
-              tma_store_2d(&tm_c, smem_cd_wg, c0, r0);
-              tma_store_2d(&tm_c, smem_cd_wg + 64 * 128, c0 + 128, r0);
-              tma_store_commit();
-            }
+            const int c0 = n0 + s * 32, r0 = m0 + cwg * 64;
+            tma_store_2d(&tm_c, smem_cd_wg, c0, r0);
+            tma_store_2d(&tm_c, smem_cd_wg + 64 * 128, c0 + 128, r0);
+            tma_store_commit();
           }
         }
       }
@@ -650,7 +689,7 @@ static int launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
                        float* cand_val = nullptr, int* cand_idx = nullptr, float* lse_part = nullptr,
                        int n_chunks = 1, const LnFold& lf = LnFold(), const ColFilter& cf = ColFilter(), int k_splits = 1,
                        int* splitk_flags = nullptr) {
-  using Cfg = GemmCfg<kCtaGroup>;
+  using Cfg = GemmCfg<kCtaGroup, kEpi>;
   auto kern = gemm_bf16_wgmma_kernel<kCtaGroup, kEpi, OutT>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set)) {
