@@ -55,6 +55,7 @@ extern "C" {
 #define SB_EPI_BIAS_RELU 1
 #define SB_EPI_BIAS_RESIDUAL 2
 #define SB_EPI_BIAS_SILU 5
+#define SB_EPI_BIAS_TANH 7
 
 typedef struct SbEncoder SbEncoder;
 
@@ -497,6 +498,56 @@ int sb_laser2_check_inputs(SbLaser2* enc, void* stream);
 int sb_lstm_recurrent(const void* G, int64_t ldg, const void* w_hh, const int32_t* cu_seqlens, const int32_t* tile_seqs,
                       int32_t num_tiles, int32_t num_dirs, void* y, int64_t ldy, float* pool_out, int64_t ldp,
                       const uint8_t* pad_mask, const uint8_t* tail_keep, float padding_value, void* stream);
+
+/* ---- BLASER 2.0: translation-quality scores from sentence embeddings ----
+ * Replaces BlaserModel.forward / featurize_input (sonar/models/blaser/model.py:82-125) of the `basic_ref` (COMET) and
+ * `basic_qe` (QE) configs (sonar/models/blaser/config.py:43-67), in eval mode (dropout off):
+ *   F.normalize each input row -> features -> [Linear -> Tanh] x num_hidden -> Linear(hidden_dims[last] -> 1)
+ * with the features (model.py:99-124)
+ *   COMET: [ref, mt, src*mt, ref*mt, |mt-src|, |mt-ref|]  (6E)      QE: [src, mt, src*mt, |mt-src|]  (4E).
+ * The features and the hidden layers but the last are bf16, the last hidden layer and the score fp32.  A pair's score does
+ * not depend on the other pairs of the call or their number, bit for bit. */
+#define SB_BLASER_COMET 0
+#define SB_BLASER_QE 1
+
+typedef struct SbBlaser SbBlaser;
+
+typedef struct SbBlaserConfig {
+  int32_t input_form;         /* SB_BLASER_COMET | SB_BLASER_QE */
+  int32_t embedding_dim;      /* E = 1024; a positive multiple of 16 with a feature width (4E QE, 6E COMET) that is a
+                               * multiple of 64 */
+  int32_t num_hidden;         /* >= 1 (the positive entries of the reference's hidden_dims) */
+  const int32_t* hidden_dims; /* HOST [num_hidden], each a positive multiple of 256 ([3072, 1536]); copied at create */
+  int32_t cta_group;          /* GEMM tiles: 0/2 = CTA pairs, 1 = single CTAs */
+  int32_t num_sms;            /* 0 = query the device */
+} SbBlaserConfig;
+
+/* HOST arrays of num_hidden + 1 DEVICE pointers (caller-owned, must outlive the handle), in the order of the module's
+ * Linear layers (mlp.<i>.weight / .bias):
+ *   w[i], i < num_hidden: bf16 [hidden_dims[i], in_i] (in_0 = the feature width)      b[i]: fp32 [hidden_dims[i]]
+ *   w[num_hidden]: fp32 [hidden_dims[num_hidden - 1]] (the output layer's single row, 16-byte aligned)  b: fp32 [1] */
+typedef struct SbBlaserWeights {
+  const void* const* w;
+  const float* const* b;
+} SbBlaserWeights;
+
+/* Allocates no device memory and does not synchronise. */
+int sb_blaser_create(const SbBlaserConfig* cfg, const SbBlaserWeights* w, SbBlaser** out);
+void sb_blaser_destroy(SbBlaser* model);
+/* Bytes of device workspace for <= max_rows pairs: max_rows * (F * 2 + max(inner hidden widths) * 2 + hidden_dims[last] * 4)
+ * plus alignment (about 1.6 GB for 65 536 pairs of `basic_ref`). */
+int sb_blaser_workspace_bytes(const SbBlaser* model, int32_t max_rows, size_t* bytes);
+/* src, mt, ref  DEVICE fp32 [rows, ld] embeddings (ld >= E, ld % 4 == 0, 16-byte aligned); ref is not read for QE and may
+ *               be NULL there
+ * scores        DEVICE fp32 [rows]
+ * Asynchronous on `stream`; never allocates; rows = 0 does nothing. */
+int sb_blaser_forward(SbBlaser* model, const float* src, const float* mt, const float* ref, int64_t ld, int32_t rows,
+                      float* scores, void* workspace, size_t workspace_bytes, void* stream);
+/* The featurization alone: out DEVICE [rows, 6E] (COMET) or [rows, 4E] (QE), fp32 (out_fp32 = 1) or bf16, of the inputs
+ * as given (normalize = 0, BlaserModel.featurize_input) or after F.normalize (normalize = 1, what forward feeds the first
+ * Linear).  E a positive multiple of 16; the other arguments as for sb_blaser_forward. */
+int sb_blaser_featurize(const float* src, const float* mt, const float* ref, int64_t ld, int32_t rows, int32_t E,
+                        int32_t input_form, int32_t normalize, void* out, int32_t out_fp32, void* stream);
 
 #ifdef __cplusplus
 }

@@ -17,3 +17,4 @@ from .text_encoder import (  # noqa: F401
 from .text_decoder import B200TextDecoderModel, SonarTextDecoderConfig, sonar_text_decoder_config  # noqa: F401,E402
 from .speech_encoder import B200SpeechEncoderModel, SonarSpeechEncoderConfig, sonar_speech_encoder_config  # noqa: F401,E402
 from .laser2 import B200LaserLstmEncoder, Laser2Config, laser2_config  # noqa: F401,E402
+from .blaser import B200BlaserModel, BlaserConfig, blaser_config, load_blaser_model  # noqa: F401,E402

@@ -14,7 +14,8 @@ _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libsonar_b200.so"
 _lib: Optional[C.CDLL] = None
 
 SB_POOL_MAX, SB_POOL_MEAN, SB_POOL_LAST, SB_POOL_ATTENTION = 1, 2, 3, 4
-SB_EPI_BIAS, SB_EPI_BIAS_RELU, SB_EPI_BIAS_RESIDUAL = 0, 1, 2
+SB_EPI_BIAS, SB_EPI_BIAS_RELU, SB_EPI_BIAS_RESIDUAL, SB_EPI_BIAS_TANH = 0, 1, 2, 7
+SB_BLASER_COMET, SB_BLASER_QE = 0, 1
 SB_ERR_INVALID, SB_ERR_CUDA, SB_ERR_DRIVER, SB_ERR_INPUT = -1, -2, -3, -4
 
 
@@ -99,6 +100,15 @@ class SbLaser2Weights(C.Structure):
     _fields_ = [("embed", C.c_void_p), ("layers", C.POINTER(SbLstmLayerWeights))]
 
 
+class SbBlaserConfig(C.Structure):
+    _fields_ = [("input_form", C.c_int32), ("embedding_dim", C.c_int32), ("num_hidden", C.c_int32),
+                ("hidden_dims", C.POINTER(C.c_int32)), ("cta_group", C.c_int32), ("num_sms", C.c_int32)]
+
+
+class SbBlaserWeights(C.Structure):
+    _fields_ = [("w", C.POINTER(C.c_void_p)), ("b", C.POINTER(C.c_void_p))]
+
+
 # name -> (restype, argtypes); must list every symbol include/sonar_b200.h declares
 _SIGNATURES = {
     "sb_last_error": (C.c_char_p, []),
@@ -172,6 +182,13 @@ _SIGNATURES = {
     "sb_lstm_recurrent": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                     C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float,
                                     C.c_void_p]),
+    "sb_blaser_create": (C.c_int, [C.POINTER(SbBlaserConfig), C.POINTER(SbBlaserWeights), C.POINTER(C.c_void_p)]),
+    "sb_blaser_destroy": (None, [C.c_void_p]),
+    "sb_blaser_workspace_bytes": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_size_t)]),
+    "sb_blaser_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
+                                    C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sb_blaser_featurize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
 }
 
 

@@ -18,7 +18,7 @@ ROOT = Path(__file__).resolve().parent
 CSRC = ROOT / "csrc"
 LIB_DIR = ROOT / "lib"
 LIB_PATH = LIB_DIR / "libsonar_b200.so"
-SOURCES = ["encoder.cu", "gemm_wgmma.cu", "gemm_skinny.cu", "attention_tc.cu", "elementwise.cu", "xsim.cu", "decoder.cu", "beam.cu", "fbank.cu", "conformer.cu", "attention_relpos_tc.cu", "latent_attention.cu", "lstm.cu"]
+SOURCES = ["encoder.cu", "gemm_wgmma.cu", "gemm_skinny.cu", "attention_tc.cu", "elementwise.cu", "xsim.cu", "decoder.cu", "beam.cu", "fbank.cu", "conformer.cu", "attention_relpos_tc.cu", "latent_attention.cu", "lstm.cu", "blaser.cu"]
 HEADERS = ["common.cuh", "attention_wgmma.cuh", "sonar_b200_internal.h", "../../include/sonar_b200.h"]
 
 NVCC_FLAGS = [

@@ -333,6 +333,12 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
           float f = fold_in ? fmaf(ln.y, fmaf(-ln.x, c, v), b) : v + b;
           if constexpr (kEpi == EPI_BIAS_RELU) f = fmaxf(f, 0.0f);
           if constexpr (kEpi == EPI_BIAS_SILU) f = silu_fast(f);
+          if constexpr (kEpi == EPI_BIAS_TANH) {
+            // tanh(f), written in silu_fast's h = f / 2 form: h + h == f for every normal f, and with it ptxas allocates
+            // the four tanh instantiations without spills (a plain tanh_approx(f) spills 8-48 bytes at the 168-register cap)
+            const float h = 0.5f * f;
+            f = tanh_approx(h + h);
+          }
           if constexpr (kEpi == EPI_BIAS_RESIDUAL) {
             if (grow < M) {
               if constexpr (sizeof(OutT) == 4) f += reinterpret_cast<const float*>(residual)[(long long)grow * ldr + col];
@@ -854,6 +860,7 @@ int gemm_bf16(const GemmArgs& g, cudaStream_t stream) {
     case EPI_BIAS: SB_DISPATCH(CG, EPI_BIAS, T);                            \
     case EPI_BIAS_RELU: SB_DISPATCH(CG, EPI_BIAS_RELU, T);                  \
     case EPI_BIAS_SILU: SB_DISPATCH(CG, EPI_BIAS_SILU, T);                  \
+    case EPI_BIAS_TANH: SB_DISPATCH(CG, EPI_BIAS_TANH, T);                  \
     case EPI_BIAS_RESIDUAL: SB_DISPATCH(CG, EPI_BIAS_RESIDUAL, T);          \
     case EPI_BIAS_ACCUM: SB_DISPATCH(CG, EPI_BIAS_ACCUM, float);            \
     case EPI_BIAS_RESIDUAL_STATS: SB_DISPATCH(CG, EPI_BIAS_RESIDUAL_STATS, float); \

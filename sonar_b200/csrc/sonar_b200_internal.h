@@ -19,9 +19,10 @@ namespace sb {
 // Bit-identical to EPI_BIAS_RESIDUAL: both compute fl32(x + fl32(acc + bias)).
 // EPI_TOPK (internal): no C at all -- the epilogue keeps a running per-row top-k of the product (xsim mining).
 // EPI_BIAS_SILU: x*sigmoid(x) (the Conformer's swish FFN activation)
+// EPI_BIAS_TANH: tanh(x) (BLASER's hidden layers)
 // EPI_BIAS_RESIDUAL_STATS (internal): fp32 C = residual + A.W^T + bias, plus the bf16 copy and row statistics of LnFold
 enum EpiMode { EPI_BIAS = 0, EPI_BIAS_RELU = 1, EPI_BIAS_RESIDUAL = 2, EPI_BIAS_ACCUM = 3, EPI_TOPK = 4, EPI_BIAS_SILU = 5,
-               EPI_BIAS_RESIDUAL_STATS = 6 };
+               EPI_BIAS_RESIDUAL_STATS = 6, EPI_BIAS_TANH = 7 };
 constexpr int kTopkCandidates = 16;  // bf16-similarity candidates per row handed to the exact fp64 re-rank
 enum PoolMode { POOL_MAX = 1, POOL_MEAN = 2, POOL_LAST = 3 };  // = reference `Pooling` enum values (model.py:23-27)
 

@@ -33,14 +33,15 @@ def _ptr(t: Optional[Tensor]) -> Optional[int]:
 
 def gemm_bf16(a: Tensor, w: Tensor, bias: Tensor, *, epilogue: str = "bias", residual: Optional[Tensor] = None,
               out_dtype: torch.dtype = torch.bfloat16, out: Optional[Tensor] = None, cta_group: int = 2) -> Tensor:
-    """out[M,N] = epi(a[M,K] @ w[N,K]^T + bias[N]); epilogue in {bias, relu, residual}."""
+    """out[M,N] = epi(a[M,K] @ w[N,K]^T + bias[N]); epilogue in {bias, relu, silu, tanh, residual}."""
     _need_cuda(a, w, bias, residual, out)
     assert a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and bias.dtype == torch.float32
     assert a.dim() == 2 and w.dim() == 2 and a.stride(1) == 1 and w.stride(1) == 1
     m, k = a.shape
     n = w.shape[0]
     assert w.shape[1] == k and bias.numel() == n
-    epi = {"bias": _lib.SB_EPI_BIAS, "relu": _lib.SB_EPI_BIAS_RELU, "residual": _lib.SB_EPI_BIAS_RESIDUAL, "silu": 5}[epilogue]
+    epi = {"bias": _lib.SB_EPI_BIAS, "relu": _lib.SB_EPI_BIAS_RELU, "residual": _lib.SB_EPI_BIAS_RESIDUAL, "silu": 5,
+           "tanh": _lib.SB_EPI_BIAS_TANH}[epilogue]
     if out is None:
         out = torch.empty((m, n), dtype=out_dtype, device=a.device)
     assert out.dtype in (torch.bfloat16, torch.float32) and out.stride(1) == 1
@@ -232,4 +233,22 @@ def lstm_recurrent(g: Tensor, w_hh: Tensor, cu_seqlens: Tensor, tile_seqs: Tenso
                                        tile_seqs.numel() // LSTM_TILE_ROWS, num_dirs, _ptr(y), ld, _ptr(pool_out), ld,
                                        _ptr(pad_mask), _ptr(tail_keep), padding_value, _stream())
     _lib.check(rc, "sb_lstm_recurrent")
+    return out
+
+
+def blaser_featurize(src: Tensor, mt: Tensor, ref: Optional[Tensor], input_form: str, *, normalize: bool = False,
+                     out_dtype: torch.dtype = torch.float32) -> Tensor:
+    """BLASER's feature rows of fp32 [N, E] embeddings (``sb_blaser_featurize``): COMET [ref, mt, src*mt, ref*mt,
+    |mt-src|, |mt-ref|] or QE [src, mt, src*mt, |mt-src|] (ref unused), of the rows as given or, with ``normalize``,
+    after ``F.normalize``; out_dtype fp32 or bf16."""
+    _need_cuda(src, mt, ref)
+    qe = {"COMET": False, "QE": True}[input_form]
+    for t in (src, mt) + (() if qe else (ref,)):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.shape == src.shape and t.dim() == 2
+    n, e = src.shape
+    out = torch.empty((n, (4 if qe else 6) * e), dtype=out_dtype, device=src.device)
+    rc = _lib.load().sb_blaser_featurize(src.data_ptr(), mt.data_ptr(), None if qe else ref.data_ptr(), e, n, e,
+                                         _lib.SB_BLASER_QE if qe else _lib.SB_BLASER_COMET, int(normalize),
+                                         out.data_ptr(), int(out_dtype == torch.float32), _stream())
+    _lib.check(rc, "sb_blaser_featurize")
     return out
