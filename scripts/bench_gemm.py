@@ -1,19 +1,19 @@
 """Where the wgmma GEMM's time goes at the text encoder's shapes (M = 4096 x 128 tokens), on one GPU.
 
 Default mode, one JSON line:
-  * ``shapes``: the four GEMMs of an encoder layer through ``ops.gemm_bf16`` (cta_group 2) -- QKV (N 3072, bias, bf16 out),
-    out-projection (N 1024, fp32 ``x += ...``), FFN1 (N 8192, bias + ReLU, bf16 out), FFN2 (N 1024, K 8192, fp32
-    ``x += ...``) -- and ``torch.nn.functional.linear`` in bf16 (cuBLAS) on the same operands as the yardstick for what
-    this card reaches under its power limit.
+  * ``shapes``: the four GEMMs of an encoder layer through ``ops.gemm_bf16`` (``--cta-group``, default 2) -- QKV
+    (N 3072, bias, bf16 out), out-projection (N 1024, fp32 ``x += ...``), FFN1 (N 8192, bias + ReLU, bf16 out), FFN2
+    (N 1024, K 8192, fp32 ``x += ...``) -- and ``torch.nn.functional.linear`` in bf16 (cuBLAS) on the same operands
+    as the yardstick for what this card reaches under its power limit.
   * ``k_sweep``: FFN1's M and N at K in {1024, 2048, 4096, 8192}, with the least-squares fit time = a + b K: ``a`` is the
     fixed cost per launch (the epilogues and pipeline fills of every tile), ``b`` the main-loop rate.
 Device-timed with CUDA events over ``--iters`` launches after a warm-up; the card's name, power limit and SM clock are
-read in the same call.
+read in the same call.  ``--cta-group 1`` runs independent CTAs instead of 2-CTA clusters that multicast the W tile.
 
 ``--profile DIR``: instead, one 4096 x 128 forward of the 24-layer encoder under ``torch.profiler`` (CUDA activities):
 kernel time summed per kernel name as a share of the step, the trace written under DIR.
 
-    python scripts/bench_gemm.py [--iters 10] [--out FILE]
+    python scripts/bench_gemm.py [--iters 10] [--cta-group {1,2}] [--out FILE]
     python scripts/bench_gemm.py --profile DIR
 """
 
@@ -66,15 +66,15 @@ def _operands(n: int, k: int, dev, seed: int):
     return a, w, bias
 
 
-def _shapes(ops, dev, iters: int) -> dict:
+def _shapes(ops, dev, iters: int, cta_group: int) -> dict:
     out = {}
     for i, (name, (n, k, epi, fp32)) in enumerate(SHAPES.items()):
         a, w, bias = _operands(n, k, dev, seed=i)
         c = torch.zeros((M, n), device=dev, dtype=torch.float32 if fp32 else torch.bfloat16)
         if fp32:  # x += a w^T + b in place: x grows a little per launch, the work does not change
-            fn = lambda: ops.gemm_bf16(a, w, bias, epilogue=epi, residual=c, out=c, cta_group=2)  # noqa: E731
+            fn = lambda: ops.gemm_bf16(a, w, bias, epilogue=epi, residual=c, out=c, cta_group=cta_group)  # noqa: E731
         else:
-            fn = lambda: ops.gemm_bf16(a, w, bias, epilogue=epi, out=c, cta_group=2)  # noqa: E731
+            fn = lambda: ops.gemm_bf16(a, w, bias, epilogue=epi, out=c, cta_group=cta_group)  # noqa: E731
         flop = 2.0 * M * n * k
         ms = _time(fn, iters)
         ms_cublas = _time(lambda: torch.nn.functional.linear(a, w), iters)  # bf16 out, no epilogue
@@ -86,12 +86,12 @@ def _shapes(ops, dev, iters: int) -> dict:
     return out
 
 
-def _k_sweep(ops, dev, iters: int) -> dict:
+def _k_sweep(ops, dev, iters: int, cta_group: int) -> dict:
     rows = []
     for k in SWEEP_K:
         a, w, bias = _operands(FFN, k, dev, seed=10 + k)
         c = torch.empty((M, FFN), device=dev, dtype=torch.bfloat16)
-        ms = _time(lambda: ops.gemm_bf16(a, w, bias, epilogue="relu", out=c, cta_group=2), iters)
+        ms = _time(lambda: ops.gemm_bf16(a, w, bias, epilogue="relu", out=c, cta_group=cta_group), iters)
         ms_cublas = _time(lambda: torch.nn.functional.linear(a, w), iters)
         rows.append({"K": k, "ms": ms, "TFLOPs": 2.0 * M * FFN * k / ms / 1e9, "cublas_ms": ms_cublas,
                      "cublas_TFLOPs": 2.0 * M * FFN * k / ms_cublas / 1e9})
@@ -110,14 +110,15 @@ def _k_sweep(ops, dev, iters: int) -> dict:
     return {"M": M, "N": FFN, "rows": rows, "fit": fit("ms"), "fit_cublas": fit("cublas_ms")}
 
 
-def _profile(out_dir: str) -> dict:
+def _profile(out_dir: str, cta_group: int) -> dict:
     from torch.profiler import ProfilerActivity, profile
 
     import bench
     from sonar_b200 import B200TextEncoderModel, SequenceBatch, sonar_text_encoder_config
 
     dev = torch.device("cuda:0")
-    model = B200TextEncoderModel(sonar_text_encoder_config("basic"), bench.synthetic_state_dict(dev), dev, cta_group=2)
+    model = B200TextEncoderModel(sonar_text_encoder_config("basic"), bench.synthetic_state_dict(dev), dev,
+                                 cta_group=cta_group)
     g = torch.Generator().manual_seed(1000)
     batch = SequenceBatch(torch.randint(4, bench.VOCAB, (4096, 128), generator=g).to(dev), None)
     for _ in range(2):
@@ -144,6 +145,7 @@ def _profile(out_dir: str) -> dict:
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=10)
+    ap.add_argument("--cta-group", type=int, default=2, choices=[1, 2])
     ap.add_argument("--profile", default="", metavar="DIR", help="profile one encoder step instead; trace under DIR")
     ap.add_argument("--out", default="")
     args = ap.parse_args()
@@ -155,12 +157,12 @@ def main() -> None:
 
     build.build()
     dev = torch.device("cuda:0")
-    res = {"gpu": _gpu_info(), "M": M}
+    res = {"gpu": _gpu_info(), "M": M, "cta_group": args.cta_group}
     if args.profile:
-        res["profile"] = _profile(args.profile)
+        res["profile"] = _profile(args.profile, args.cta_group)
     else:
-        res["shapes"] = _shapes(ops, dev, args.iters)
-        res["k_sweep"] = _k_sweep(ops, dev, args.iters)
+        res["shapes"] = _shapes(ops, dev, args.iters, args.cta_group)
+        res["k_sweep"] = _k_sweep(ops, dev, args.iters, args.cta_group)
     res["gpu_after"] = _gpu_info()
     line = json.dumps(res)
     print(line)

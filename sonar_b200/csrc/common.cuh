@@ -86,13 +86,17 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
+// arrive on the barrier at the same smem offset in CTA `cta` of the cluster.
+// Default semantics (.release at .cta scope): the callers release a ring slot whose wgmma reads have retired; they wrote
+// nothing the slot's producer must see, and its next writer is a TMA load ordered by the barrier phase.  The
+// `.release.cluster` form compiled to MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR before the arrive: a GPU-wide fence in every
+// consumer warp and k-block of the 2-CTA GEMM (tests/test_gemm_sass.py keeps it out of the main loops).
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n\t"
       ".reg .b32 ra;\n\t"
       "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
       "}\n" ::"r"(smem_u32(bar)),
       "r"(cta)
       : "memory");

@@ -36,8 +36,8 @@ constexpr bool epi_row_wise(int epi) { return epi == EPI_BIAS_RESIDUAL_STATS || 
 // Shared memory: the row-wise epilogues keep 3 ring stages next to their transposition buffers (2 x 17 KB); the
 // column-wise ones have no such buffer and spend the space on a 4th stage, so the producer can run 4 k-blocks of the next
 // tile ahead while the epilogue runs.  The other layout that fits, 3 stages and four staging boxes per warpgroup (a whole
-// bf16 tile, one store wait per tile), measured slower in the same run on an H100 SXM (700 W): 3.35 k against 3.39 k
-// sentences/s in bench.py, FFN1 alone 469 against 473 TFLOP/s, FFN2 510 against 523.
+// bf16 tile, one store wait per tile), measured slower in the same call on an H100 80GB HBM3 (700 W): median 4.43 k against
+// 4.48 k sentences/s over three alternating bench.py runs each, with a spread of 0.013 k and 0.033 k within each layout.
 template <int kCtaGroup, int kEpi>
 struct GemmCfg {
   static constexpr bool ROW_WISE = epi_row_wise(kEpi);
