@@ -224,6 +224,29 @@ int sb_pool(const float* x, const int32_t* cu_seqlens, int32_t B, int32_t D, con
 int sb_pool_latent_attention(const void* qt, const void* mem, const int32_t* cu_seqlens, int32_t B, int32_t Hd, int32_t D,
                              void* u, void* stream);
 
+/* The speech encoder's kernels, launched as sb_speech_encoder_forward launches them.  Packed rows: utterance b owns rows
+ * cu_seqlens[b] .. cu_seqlens[b+1] - 1 (cu_seqlens DEVICE int32 [B+1]).
+ *
+ * Transformer-XL relative-position self-attention of a Conformer block, D = 64 * H in {256, 512, 768, 1024}:
+ *   out[i] = sum_j softmax_j(((q_i + u) . k_j + (q_i + v) . p[S_center - 1 - i + j]) / 8) v_j   over the keys j of i's utterance
+ * qkv bf16 [total_tokens, 3D] (q | k | v), p bf16 [Npad, D] = r_proj of the relative-position table (row k <-> relative
+ * position S_center - 1 - k), u_bias / v_bias fp32 [D], out bf16 [total_tokens, D].  S_center = the longest utterance,
+ * Npad = roundup(2 * S_center - 1, 256).  impl 0 = the wgmma kernel (B <= 2047; qu, qv bf16 [total_tokens, D] scratch),
+ * impl 1 = the mma.sync kernel (vp fp32 [H, Npad] scratch). */
+int sb_attention_relpos(const void* qkv, const void* p, const float* u_bias, const float* v_bias, const int32_t* cu_seqlens,
+                        int32_t B, int32_t H, int64_t total_tokens, int32_t Npad, int32_t S_center, int32_t impl, void* qu,
+                        void* qv, float* vp, void* out, void* stream);
+/* The convolution module between its pointwise convolutions: g bf16 [total, 2D] (value | gate) -> out bf16 [total, D] =
+ * SiLU(bn_scale * depthwise_conv(value * sigmoid(gate)) + bn_shift), 31 taps dw fp32 [D, 31], zero outside each utterance;
+ * max_len = the longest utterance, D a multiple of 64. */
+int sb_conformer_conv(const void* g, const int32_t* cu_seqlens, int32_t B, int32_t max_len, int32_t D, const float* dw,
+                      const float* bn_scale, const float* bn_shift, void* out, void* stream);
+/* The w2v-BERT frontend's first step: row cu_seqlens[b] + t of out (bf16 [total, 192]) = LayerNorm(160) of fbank frames
+ * 2t, 2t+1 of utterance b (fbank DEVICE fp32 [B, padded_frames, 80]), columns 160..191 zero; max_len = the longest
+ * utterance (2 * max_len <= padded_frames). */
+int sb_speech_frontend(const float* fbank, int32_t padded_frames, const int32_t* cu_seqlens, int32_t B, int32_t max_len,
+                       const float* gamma, const float* beta, float eps, void* out, void* stream);
+
 /* ---- embedding -> text decoder, one incremental step at a time (BASELINE.json config 4) ----
  * Replaces ConditionalTransformerDecoderModel.decode + project (sonar/nn/conditional_decoder_model.py:60-94,
  * built by SonarTextDecoderFactory, sonar/models/sonar_text/factory.py:229-315) as driven by fairseq2's

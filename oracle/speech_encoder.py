@@ -61,6 +61,34 @@ def rel_pos_table(seq_len: int, dim: int) -> Tensor:
     return torch.cat([torch.flip(p, [0]), n[1:]], dim=0)
 
 
+def relpos_attention(q: Tensor, k: Tensor, v: Tensor, r: Tensor, u_bias: Tensor, v_bias: Tensor, key_ok: Tensor) -> Tensor:
+    """The Transformer-XL relative-position attention core of a Conformer block: q, k, v [B, S, H, hd]; r [2S-1, H, hd] =
+    r_proj(rel_pos_table(S)), row c <-> relative position S-1-c; u_bias, v_bias [H, hd]; key_ok [B, S] -> [B, S, H*hd] =
+    softmax_j(((q_i+u).k_j + (q_i+v).r[S-1-i+j]) / sqrt(hd), keys with key_ok False excluded) . v."""
+    b, s, H, hd = q.shape
+    k, v = k.transpose(1, 2), v.transpose(1, 2)  # [B,H,S,hd]
+    qu = (q + u_bias).transpose(1, 2)
+    qv = (q + v_bias).transpose(1, 2)
+    ac = qu @ k.transpose(-2, -1)
+    bd_full = qv @ r.permute(1, 2, 0)  # [B,H,S,2S-1]; column c <-> relative position S-1-c
+    idx = (s - 1) - torch.arange(s)[:, None] + torch.arange(s)[None, :]  # column for (i,j): relpos i-j
+    bd = torch.gather(bd_full, 3, idx[None, None].expand(b, H, s, s))
+    scores = (ac + bd) / math.sqrt(hd)
+    scores = scores.masked_fill(~key_ok[:, None, None, :], -torch.inf)
+    return (torch.softmax(scores, dim=-1) @ v).transpose(1, 2).reshape(b, s, H * hd)
+
+
+def conv_module_middle(y: Tensor, dw: Tensor, bn_mean: Tensor, bn_var: Tensor, bn_weight: Tensor, bn_bias: Tensor,
+                       bn_eps: float) -> Tensor:
+    """The convolution module between its pointwise convolutions: y [B, 2D, S] (pointwise_conv1 output, zero at padded
+    positions) -> GLU -> depthwise conv (dw [D, 1, k], zero padding k//2) -> BatchNorm (running statistics) -> SiLU
+    -> [B, D, S]."""
+    y = F.glu(y, dim=1)
+    y = F.conv1d(y, dw, padding=dw.shape[-1] // 2, groups=y.shape[1])
+    y = F.batch_norm(y, bn_mean, bn_var, bn_weight, bn_bias, False, 0.0, bn_eps)
+    return F.silu(y)
+
+
 def make_synthetic_speech_state_dict(cfg: OracleSpeechConfig, seed: int = 3, std: float = 0.02) -> Dict[str, Tensor]:
     g = torch.Generator().manual_seed(seed)
     d, f, H = cfg.model_dim, cfg.ffn_inner_dim, cfg.num_heads
@@ -139,27 +167,18 @@ class OracleSpeechEncoder:
         y = lnorm(x, "self_attn_layer_norm")
         a = p + "self_attn."
         q = F.linear(y, sd[a + "q_proj.weight"], sd[a + "q_proj.bias"]).view(b, s, H, hd)
-        k = F.linear(y, sd[a + "k_proj.weight"], sd[a + "k_proj.bias"]).view(b, s, H, hd).transpose(1, 2)
-        v = F.linear(y, sd[a + "v_proj.weight"], sd[a + "v_proj.bias"]).view(b, s, H, hd).transpose(1, 2)
+        k = F.linear(y, sd[a + "k_proj.weight"], sd[a + "k_proj.bias"]).view(b, s, H, hd)
+        v = F.linear(y, sd[a + "v_proj.weight"], sd[a + "v_proj.bias"]).view(b, s, H, hd)
         r = F.linear(rel_pos_table(s, d), sd[a + "sdpa.r_proj.weight"]).view(2 * s - 1, H, hd)  # [2S-1,H,hd]
-        qu = (q + sd[a + "sdpa.u_bias"]).transpose(1, 2)  # [B,H,S,hd]
-        qv = (q + sd[a + "sdpa.v_bias"]).transpose(1, 2)
-        ac = qu @ k.transpose(-2, -1)
-        bd_full = qv @ r.permute(1, 2, 0)  # [B,H,S,2S-1]; column c <-> relative position S-1-c
-        idx = (s - 1) - torch.arange(s)[:, None] + torch.arange(s)[None, :]  # column for (i,j): relpos i-j
-        bd = torch.gather(bd_full, 3, idx[None, None].expand(b, H, s, s))
-        scores = (ac + bd) / math.sqrt(hd)
-        scores = scores.masked_fill(~key_ok[:, None, None, :], -torch.inf)
-        o = (torch.softmax(scores, dim=-1) @ v).transpose(1, 2).reshape(b, s, d)
+        o = relpos_attention(q, k, v, r, sd[a + "sdpa.u_bias"], sd[a + "sdpa.v_bias"], key_ok)
         x = x + F.linear(o, sd[a + "output_proj.weight"], sd[a + "output_proj.bias"])
         # --- convolution module ---
         y = lnorm(x, "conv_layer_norm")
         y = y.masked_fill(~key_ok[:, :, None], 0.0).transpose(1, 2)  # [B,D,S]
-        y = F.glu(F.conv1d(y, sd[p + "conv.pointwise_conv1.weight"]), dim=1)
-        y = F.conv1d(y, sd[p + "conv.depthwise_conv.weight"], padding=cfg.conv_kernel // 2, groups=d)
-        y = F.batch_norm(y, sd[p + "conv.batch_norm.running_mean"], sd[p + "conv.batch_norm.running_var"],
-                         sd[p + "conv.batch_norm.weight"], sd[p + "conv.batch_norm.bias"], False, 0.0, cfg.bn_eps)
-        y = F.conv1d(F.silu(y), sd[p + "conv.pointwise_conv2.weight"]).transpose(1, 2)
+        bn = p + "conv.batch_norm."
+        y = conv_module_middle(F.conv1d(y, sd[p + "conv.pointwise_conv1.weight"]), sd[p + "conv.depthwise_conv.weight"],
+                               sd[bn + "running_mean"], sd[bn + "running_var"], sd[bn + "weight"], sd[bn + "bias"], cfg.bn_eps)
+        y = F.conv1d(y, sd[p + "conv.pointwise_conv2.weight"]).transpose(1, 2)
         x = x + y
         x = x + 0.5 * ffn(lnorm(x, "ffn2_layer_norm"), "ffn2")
         return lnorm(x, "layer_norm")

@@ -136,6 +136,11 @@ _SIGNATURES = {
                           C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "sb_pool_latent_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                            C.c_void_p, C.c_void_p]),
+    "sb_attention_relpos": (C.c_int, [C.c_void_p] * 5 + [C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int32] +
+                            [C.c_void_p] * 5),
+    "sb_conformer_conv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 5),
+    "sb_speech_frontend": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                     C.c_float, C.c_void_p, C.c_void_p]),
     "sb_decoder_create": (C.c_int, [C.POINTER(SbDecoderConfig), C.POINTER(SbDecoderWeights), C.POINTER(C.c_void_p)]),
     "sb_decoder_destroy": (None, [C.c_void_p]),
     "sb_decoder_workspace_bytes": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]),

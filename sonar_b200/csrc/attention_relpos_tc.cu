@@ -37,7 +37,7 @@ constexpr int kOffQu = 0, kOffQv = kTile, kOffK = 2 * kTile, kOffPlo = 3 * kTile
 constexpr int kBLd = 197;                         // floats per row of a warpgroup's Bw buffer (192 + skew padding)
 constexpr int kBBytes = 64 * kBLd * 4;            // per consumer warpgroup
 constexpr int kBarBytes = 512;
-constexpr int kMaxBatch = 2047;                   // cu_seqlens and the query-tile prefix are staged in shared memory
+constexpr int kMaxBatch = kRelposTcMaxBatch;
 constexpr int kSmemBytes = kOperandBytes + 2 * kBBytes + kBarBytes + 2 * (kMaxBatch + 1) * 4 + 1024;
 constexpr int kThreads = 384;
 static_assert(kSmemBytes <= 232448, "shared memory budget of one sm_90 block");

@@ -475,6 +475,59 @@ glu_dwconv_kernel(const __nv_bfloat16* __restrict__ g, const int32_t* __restrict
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// launches: the speech encoder's forward and the kernel-level entry points below call the same functions
+// ---------------------------------------------------------------------------------------------
+// p rows of the relative-position table for a batch whose longest utterance has smax positions
+int npad_of(int smax) { return ((2 * smax - 1) + 255) / 256 * 256; }
+
+// fbank fp32 [B, padded_frames, 80] -> out bf16 [T, 192]
+int speech_frontend(const float* fbank, int padded_frames, const int32_t* cu, int B, int max_len, const float* gamma,
+                    const float* beta, float eps, __nv_bfloat16* out, cudaStream_t stream) {
+  frontend_ln_kernel<<<dim3((unsigned)B, (unsigned)((max_len + 7) / 8)), 256, 0, stream>>>(fbank, padded_frames, cu, gamma,
+                                                                                          beta, eps, out);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return SB_OK;
+}
+
+// g bf16 [T, 2D] (value | gate) -> out bf16 [T, D]: GLU -> depthwise conv (31 taps) -> BatchNorm scale / shift -> SiLU
+int conformer_conv(const __nv_bfloat16* g, const int32_t* cu, int B, int max_len, int D, const float* dw, const float* bn_scale,
+                   const float* bn_shift, __nv_bfloat16* out, cudaStream_t stream) {
+  static bool carve_set[64] = {};
+  if (first_use_on_device(carve_set))  // 5 CTAs x 32 KB of static shared memory per SM: ask for the large carve-out
+    SB_CUDA_CHECK(cudaFuncSetAttribute(glu_dwconv_kernel<31>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                       cudaSharedmemCarveoutMaxShared));
+  glu_dwconv_kernel<31><<<dim3((unsigned)((max_len + 63) / 64), (unsigned)(D / 64), (unsigned)B), 128, 0, stream>>>(
+      g, cu, D, dw, bn_scale, bn_shift, out);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return SB_OK;
+}
+
+// Relative-position attention: impl 0 = the wgmma kernel (attention_relpos_tc.cu, B <= kRelposTcMaxBatch), impl 1 = v.p
+// (relpos_bias_kernel into vp [H, Npad]) followed by the mma.sync kernel.  qkv [T, 3D], p [Npad, D], out [T, D] bf16;
+// qu / qv [T, D] bf16 scratch of impl 0; S_center = the batch's longest utterance.
+int attention_relpos(const __nv_bfloat16* qkv, const __nv_bfloat16* p, const float* u_bias, const float* v_bias,
+                     const int32_t* cu, int B, int H, long long T, int Npad, int S_center, int impl, __nv_bfloat16* qu,
+                     __nv_bfloat16* qv, float* vp, __nv_bfloat16* out, int num_sms, cudaStream_t stream) {
+  if (impl == 0)
+    return attention_relpos_tc(qkv, p, u_bias, v_bias, cu, B, H, T, Npad, S_center, qu, qv, out, num_sms, stream);
+  static bool attr_set[64] = {};
+  if (first_use_on_device(attr_set))
+    SB_CUDA_CHECK(cudaFuncSetAttribute(attention_relpos_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRpSmem));
+  const int D = H * 64;
+  // TMA views: 64 x 64 boxes of the packed qkv rows [T, 3D] and of the projected table [Npad, D]
+  CUtensorMap tm_qkv, tm_p;
+  int rc;
+  if ((rc = make_tmap_2d(&tm_qkv, qkv, 2, T, 3ll * D, 3ll * D, 64, 64))) return rc;
+  if ((rc = make_tmap_2d(&tm_p, p, 2, Npad, D, D, 64, 64))) return rc;
+  relpos_bias_kernel<<<dim3((unsigned)((Npad + 7) / 8), (unsigned)H), 256, 0, stream>>>(p, v_bias, Npad, H, vp);
+  SB_CUDA_CHECK(cudaGetLastError());
+  attention_relpos_kernel<<<dim3((unsigned)((S_center + 127) / 128), (unsigned)H, (unsigned)B), kRpThreads, kRpSmem, stream>>>(
+      tm_qkv, tm_p, cu, H, u_bias, vp, Npad, S_center, out);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return SB_OK;
+}
+
 }  // namespace
 }  // namespace sb
 
@@ -502,8 +555,6 @@ struct SpWs {
   AttentionPooler::Ws pool;
   size_t bytes;
 };
-
-int npad_of(int smax) { return ((2 * smax - 1) + 255) / 256 * 256; }
 
 SpWs carve_sp(const SbSpeechEncoder* e, int B, long long T, int smax, void* base) {
   const size_t D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, H = e->cfg.num_heads;
@@ -613,14 +664,8 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   const int D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, H = e->cfg.num_heads;
   const float eps = e->cfg.ln_eps;
-  static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set)) {
-    SB_CUDA_CHECK(cudaFuncSetAttribute(attention_relpos_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRpSmem));
-  }
-  // TMA views for the rel-pos attention: 64 x 64 boxes of the packed qkv rows [T, 3D] and of the projected table [Npad, D]
-  CUtensorMap tm_qkv, tm_p;
-  if ((rc = make_tmap_2d(&tm_qkv, w.big, 2, T, 3ll * D, 3ll * D, 64, 64))) return rc;
-  if ((rc = make_tmap_2d(&tm_p, w.p, 2, Npad, D, D, 64, 64))) return rc;
+  // the mma.sync kernel (A/B runs, second implementation in the tests) is the only one for more than 2047 utterances
+  const int attn_impl = (e->cfg.attn_impl == 1 || B > kRelposTcMaxBatch) ? 1 : 0;
   // every GEMM may take the weight-streaming path (as the pooler's do)
   auto gemm = [&](const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int fp32,
                   const float* bias, int M, int N, int K, int epi) {
@@ -629,9 +674,8 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
     return gemm_bf16(g, stream);
   };
   // ---- frontend ----
-  frontend_ln_kernel<<<dim3((unsigned)B, (unsigned)((smax + 7) / 8)), 256, 0, stream>>>(
-      fbank, padded_frames, cu_dev, e->w.front_ln_g, e->w.front_ln_b, eps, w.a192);
-  SB_CUDA_CHECK(cudaGetLastError());
+  if ((rc = speech_frontend(fbank, padded_frames, cu_dev, B, smax, e->w.front_ln_g, e->w.front_ln_b, eps, w.a192, stream)))
+    return rc;
   if ((rc = gemm(w.a192, kFeatPad, e->w.front_w, kFeatPad, w.x, D, 1, e->w.front_b, (int)T, D, kFeatPad, EPI_BIAS))) return rc;
   // ---- conformer blocks ----
   for (int li = 0; li < e->cfg.num_layers; ++li) {
@@ -644,30 +688,14 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
     if ((rc = layernorm_bf16(w.x, L.attn_ln_g, L.attn_ln_b, eps, w.h, T, D, stream))) return rc;
     if ((rc = gemm(w.h, D, L.wqkv, D, w.big, 3 * D, 0, L.bqkv, (int)T, 3 * D, D, EPI_BIAS))) return rc;
     if ((rc = gemm(relpos_table, D, L.wr, D, w.p, D, 0, e->w.zeros, Npad, D, D, EPI_BIAS))) return rc;
-    if (e->cfg.attn_impl == 1 || B > 2047) {  // mma.sync kernel (A/B runs, second implementation in the tests)
-      relpos_bias_kernel<<<dim3((unsigned)((Npad + 7) / 8), (unsigned)H), 256, 0, stream>>>(w.p, L.v_bias, Npad, H, w.vp);
-      SB_CUDA_CHECK(cudaGetLastError());
-      attention_relpos_kernel<<<dim3((unsigned)((smax + 127) / 128), (unsigned)H, (unsigned)B), kRpThreads, kRpSmem, stream>>>(
-          tm_qkv, tm_p, cu_dev, H, L.u_bias, w.vp, Npad, smax, w.h);
-      SB_CUDA_CHECK(cudaGetLastError());
-    } else {  // wgmma (attention_relpos_tc.cu)
-      if ((rc = attention_relpos_tc(w.big, w.p, L.u_bias, L.v_bias, cu_dev, B, H, T, Npad, smax, w.qu, w.qv, w.h, e->num_sms,
-                                    stream)))
-        return rc;
-    }
+    if ((rc = attention_relpos(w.big, w.p, L.u_bias, L.v_bias, cu_dev, B, H, T, Npad, smax, attn_impl, w.qu, w.qv, w.vp, w.h,
+                               e->num_sms, stream)))
+      return rc;
     if ((rc = gemm(w.h, D, L.wo, D, w.x, D, 1, L.bo, (int)T, D, D, EPI_BIAS_RESIDUAL))) return rc;
     // (c) convolution module
     if ((rc = layernorm_bf16(w.x, L.conv_ln_g, L.conv_ln_b, eps, w.h, T, D, stream))) return rc;
     if ((rc = gemm(w.h, D, L.pw1, D, w.big, 2 * D, 0, e->w.zeros, (int)T, 2 * D, D, EPI_BIAS))) return rc;
-    {
-      static bool carve_set[64] = {};
-      if (first_use_on_device(carve_set))  // 5 CTAs x 32 KB of static shared memory per SM: ask for the large carve-out
-        SB_CUDA_CHECK(cudaFuncSetAttribute(glu_dwconv_kernel<31>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                           cudaSharedmemCarveoutMaxShared));
-    }
-    glu_dwconv_kernel<31><<<dim3((unsigned)((smax + 63) / 64), (unsigned)(D / 64), (unsigned)B), 128, 0, stream>>>(
-        w.big, cu_dev, D, L.dw, L.bn_scale, L.bn_shift, w.h);
-    SB_CUDA_CHECK(cudaGetLastError());
+    if ((rc = conformer_conv(w.big, cu_dev, B, smax, D, L.dw, L.bn_scale, L.bn_shift, w.h, stream))) return rc;
     if ((rc = gemm(w.h, D, L.pw2, D, w.x, D, 1, e->w.zeros, (int)T, D, D, EPI_BIAS_RESIDUAL))) return rc;
     // (d) half-step FFN 2
     if ((rc = layernorm_bf16(w.x, L.ffn2_ln_g, L.ffn2_ln_b, eps, w.h, T, D, stream))) return rc;
@@ -680,6 +708,56 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
   if ((rc = layernorm_dual(w.x, e->w.final_ln_g, e->w.final_ln_b, eps, w.x, w.h, T, D, stream))) return rc;
   if (encoded_packed) SB_CUDA_CHECK(cudaMemcpyAsync(encoded_packed, w.x, sizeof(float) * (size_t)T * D, cudaMemcpyDeviceToDevice, stream));
   return e->pooler.forward(w.pool, w.h, cu_dev, B, out, stream);
+}
+
+int sb_attention_relpos(const void* qkv, const void* p, const float* u_bias, const float* v_bias, const int32_t* cu_seqlens,
+                        int32_t B, int32_t H, int64_t total_tokens, int32_t Npad, int32_t S_center, int32_t impl, void* qu,
+                        void* qv, float* vp, void* out, void* stream) {
+  if (!qkv || !p || !u_bias || !v_bias || !cu_seqlens || !out || (impl == 0 && (!qu || !qv)) || (impl == 1 && !vp)) {
+    set_last_error("sb_attention_relpos: null argument");
+    return SB_ERR_INVALID;
+  }
+  const int D = 64 * H;
+  if (impl < 0 || impl > 1 || B <= 0 || B > 65535 || total_tokens <= 0 || S_center <= 0 || H <= 0 || D % 256 != 0 || D > 1024 ||
+      Npad != npad_of(S_center)) {
+    set_last_error("sb_attention_relpos: bad argument (impl %d, B %d, H %d, T %lld, Npad %d, S_center %d)", impl, B, H,
+                   (long long)total_tokens, Npad, S_center);
+    return SB_ERR_INVALID;
+  }
+  int sms = 0;
+  if (int rc = require_hopper("sb_attention_relpos", &sms)) return rc;
+  return attention_relpos(static_cast<const __nv_bfloat16*>(qkv), static_cast<const __nv_bfloat16*>(p), u_bias, v_bias,
+                          cu_seqlens, B, H, total_tokens, Npad, S_center, impl, static_cast<__nv_bfloat16*>(qu),
+                          static_cast<__nv_bfloat16*>(qv), vp, static_cast<__nv_bfloat16*>(out), sms,
+                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sb_conformer_conv(const void* g, const int32_t* cu_seqlens, int32_t B, int32_t max_len, int32_t D, const float* dw,
+                      const float* bn_scale, const float* bn_shift, void* out, void* stream) {
+  if (!g || !cu_seqlens || !dw || !bn_scale || !bn_shift || !out) {
+    set_last_error("sb_conformer_conv: null argument");
+    return SB_ERR_INVALID;
+  }
+  if (B <= 0 || B > 65535 || max_len <= 0 || D <= 0 || D % 64 != 0) {
+    set_last_error("sb_conformer_conv: bad argument (B %d, max_len %d, D %d)", B, max_len, D);
+    return SB_ERR_INVALID;
+  }
+  return conformer_conv(static_cast<const __nv_bfloat16*>(g), cu_seqlens, B, max_len, D, dw, bn_scale, bn_shift,
+                        static_cast<__nv_bfloat16*>(out), reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sb_speech_frontend(const float* fbank, int32_t padded_frames, const int32_t* cu_seqlens, int32_t B, int32_t max_len,
+                       const float* gamma, const float* beta, float eps, void* out, void* stream) {
+  if (!fbank || !cu_seqlens || !gamma || !beta || !out) {
+    set_last_error("sb_speech_frontend: null argument");
+    return SB_ERR_INVALID;
+  }
+  if (B <= 0 || B > 65535 || max_len <= 0 || 2ll * max_len > padded_frames) {
+    set_last_error("sb_speech_frontend: bad argument (B %d, max_len %d, padded_frames %d)", B, max_len, padded_frames);
+    return SB_ERR_INVALID;
+  }
+  return speech_frontend(fbank, padded_frames, cu_seqlens, B, max_len, gamma, beta, eps, static_cast<__nv_bfloat16*>(out),
+                         reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

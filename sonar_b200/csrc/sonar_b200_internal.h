@@ -221,7 +221,9 @@ int attention_packed(const __nv_bfloat16* qkv, const int32_t* cu_seqlens, int B,
                      __nv_bfloat16* out, cudaStream_t stream);
 
 // Transformer-XL relative-position attention of the Conformer blocks on wgmma (attention_relpos_tc.cu):
-// score(i,j) = ((q_i+u).k_j + (q_i+v).p[S_center-1-i+j]) / 8; qu / qv = [T, D] bf16 scratch for the biased queries
+// score(i,j) = ((q_i+u).k_j + (q_i+v).p[S_center-1-i+j]) / 8; qu / qv = [T, D] bf16 scratch for the biased queries.
+// At most kRelposTcMaxBatch utterances: cu_seqlens and the query-tile prefix are staged in shared memory.
+constexpr int kRelposTcMaxBatch = 2047;
 int attention_relpos_tc(const __nv_bfloat16* qkv, const __nv_bfloat16* p, const float* u_bias, const float* v_bias,
                         const int32_t* cu_seqlens, int B, int H, long long total_tokens, int Npad, int S_center,
                         __nv_bfloat16* qu, __nv_bfloat16* qv, __nv_bfloat16* out, int num_sms, cudaStream_t stream);

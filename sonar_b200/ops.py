@@ -13,6 +13,7 @@ import torch
 from torch import Tensor
 
 from . import _lib
+from .speech_encoder import relpos_rows
 
 POOLING_MODES = {"max": _lib.SB_POOL_MAX, "mean": _lib.SB_POOL_MEAN, "last": _lib.SB_POOL_LAST}
 
@@ -192,6 +193,83 @@ def pool_latent_attention(qt: Tensor, mem: Tensor, cu_seqlens: Tensor) -> Tensor
                                               u.data_ptr(), _stream())
     _lib.check(rc, "sb_pool_latent_attention")
     return u
+
+
+RELPOS_IMPLS = {"wgmma": 0, "mma_sync": 1}
+
+
+def _out_rows(out: Optional[Tensor], t: int, d: int, device) -> Tensor:
+    if out is None:
+        return torch.empty((t, d), dtype=torch.bfloat16, device=device)
+    assert out.dtype == torch.bfloat16 and out.shape == (t, d) and out.is_contiguous()
+    return out
+
+
+def attention_relpos(qkv: Tensor, p: Tensor, u_bias: Tensor, v_bias: Tensor, cu_seqlens: Tensor, num_heads: int, *,
+                     impl: str = "wgmma", out: Optional[Tensor] = None) -> Tensor:
+    """The Conformer's Transformer-XL relative-position self-attention over packed utterances (``sb_attention_relpos``):
+    qkv bf16 [T, 3D] (q | k | v), p bf16 [Npad, D] (row k = r_proj of relative position S_center - 1 - k, S_center = the
+    longest utterance, Npad = ``relpos_rows(S_center)``), u_bias / v_bias fp32 [D], cu_seqlens int32 [B+1] -> bf16 [T, D];
+    ``impl`` "wgmma" (at most 2047 utterances) or "mma_sync"."""
+    _need_cuda(qkv, p, u_bias, v_bias, cu_seqlens, out)
+    d = 64 * num_heads
+    t = qkv.shape[0]
+    assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and qkv.shape == (t, 3 * d)
+    assert u_bias.dtype == torch.float32 and v_bias.dtype == torch.float32 and u_bias.numel() == v_bias.numel() == d
+    assert cu_seqlens.dtype == torch.int32
+    s_center = int(cu_seqlens.cpu().diff().max())
+    npad = relpos_rows(s_center)
+    assert p.dtype == torch.bfloat16 and p.is_contiguous() and p.shape == (npad, d), (tuple(p.shape), npad)
+    out = _out_rows(out, t, d, qkv.device)
+    code = RELPOS_IMPLS[impl]
+    qu = qv = vp = None
+    if code == 0:
+        qu = torch.empty((t, d), dtype=torch.bfloat16, device=qkv.device)
+        qv = torch.empty_like(qu)
+    else:
+        vp = torch.empty((num_heads, npad), dtype=torch.float32, device=qkv.device)
+    rc = _lib.load().sb_attention_relpos(qkv.data_ptr(), p.data_ptr(), u_bias.data_ptr(), v_bias.data_ptr(),
+                                         cu_seqlens.data_ptr(), cu_seqlens.numel() - 1, num_heads, t, npad, s_center, code,
+                                         _ptr(qu), _ptr(qv), _ptr(vp), out.data_ptr(), _stream())
+    _lib.check(rc, "sb_attention_relpos")
+    return out
+
+
+def conformer_conv(g: Tensor, cu_seqlens: Tensor, dw: Tensor, bn_scale: Tensor, bn_shift: Tensor, *,
+                   out: Optional[Tensor] = None) -> Tensor:
+    """The Conformer convolution module between its pointwise convolutions (``sb_conformer_conv``): g bf16 [T, 2D]
+    (value | gate) -> bf16 [T, D] = SiLU(bn_scale * depthwise_conv(value * sigmoid(gate)) + bn_shift), dw fp32 [D, 31],
+    zero padding at each utterance's ends."""
+    _need_cuda(g, cu_seqlens, dw, bn_scale, bn_shift, out)
+    t, d2 = g.shape
+    d = d2 // 2
+    assert g.dtype == torch.bfloat16 and g.is_contiguous() and cu_seqlens.dtype == torch.int32
+    assert dw.dtype == torch.float32 and dw.is_contiguous() and dw.shape == (d, 31)
+    assert bn_scale.dtype == bn_shift.dtype == torch.float32 and bn_scale.numel() == bn_shift.numel() == d
+    max_len = int(cu_seqlens.cpu().diff().max())
+    out = _out_rows(out, t, d, g.device)
+    rc = _lib.load().sb_conformer_conv(g.data_ptr(), cu_seqlens.data_ptr(), cu_seqlens.numel() - 1, max_len, d, dw.data_ptr(),
+                                       bn_scale.data_ptr(), bn_shift.data_ptr(), out.data_ptr(), _stream())
+    _lib.check(rc, "sb_conformer_conv")
+    return out
+
+
+def speech_frontend(fbank: Tensor, cu_seqlens: Tensor, gamma: Tensor, beta: Tensor, eps: float = 1e-5, *,
+                    out: Optional[Tensor] = None) -> Tensor:
+    """The speech frontend's frame stacking and LayerNorm (``sb_speech_frontend``): fbank fp32 [B, padded_frames, 80],
+    cu_seqlens int32 [B+1] of positions (= frames // 2) -> bf16 [T, 192], row cu[b] + t = LayerNorm(160) of frames 2t, 2t+1,
+    columns 160..191 zero."""
+    _need_cuda(fbank, cu_seqlens, gamma, beta, out)
+    assert fbank.dtype == torch.float32 and fbank.is_contiguous() and fbank.dim() == 3 and fbank.shape[2] == 80
+    assert gamma.dtype == beta.dtype == torch.float32 and gamma.numel() == beta.numel() == 160
+    assert cu_seqlens.dtype == torch.int32 and cu_seqlens.numel() == fbank.shape[0] + 1
+    cu = cu_seqlens.cpu()
+    max_len, t = int(cu.diff().max()), int(cu[-1])
+    out = _out_rows(out, t, 192, fbank.device)
+    rc = _lib.load().sb_speech_frontend(fbank.data_ptr(), fbank.shape[1], cu_seqlens.data_ptr(), fbank.shape[0], max_len,
+                                        gamma.data_ptr(), beta.data_ptr(), eps, out.data_ptr(), _stream())
+    _lib.check(rc, "sb_speech_frontend")
+    return out
 
 
 LSTM_TILE_ROWS = 64  # sequences per tile of the LSTM recurrent kernel

@@ -53,6 +53,12 @@ def sonar_speech_encoder_config(arch: str = "english", **overrides) -> SonarSpee
     return dataclasses.replace(cfg, **overrides)
 
 
+def relpos_rows(max_len: int) -> int:
+    """Rows of the relative-position table for a batch whose longest utterance has ``max_len`` positions: 2*max_len-1
+    rounded up to a multiple of 256."""
+    return ((2 * max_len - 1) + 255) // 256 * 256
+
+
 def relative_position_table(max_len: int, dim: int, rows: int) -> Tensor:
     """fp32 [rows, dim]: row k (< 2*max_len-1) = sinusoid of relative position (max_len-1-k), interleaved sin/cos;
     remaining rows zero.  (fairseq2 ``RelativePositionalEncoding`` / Transformer-XL; SURVEY App. B.2.)"""
@@ -145,7 +151,7 @@ class B200SpeechEncoderModel(EngineModel):
         if min(lens) < 1:
             raise ValueError("every utterance needs at least 2 fbank frames")
         smax, total = max(lens), sum(lens)
-        rows = ((2 * smax - 1) + 255) // 256 * 256
+        rows = relpos_rows(smax)
         if rows > 8192:
             raise ValueError("utterance too long for the relative-position workspace")
         if smax not in self._relpos:
