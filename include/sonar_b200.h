@@ -317,6 +317,36 @@ int sb_decoder_step(SbDecoder* dec, const int64_t* tokens, const int32_t* table,
                     void* stream);
 int sb_decoder_check_inputs(SbDecoder* dec, void* workspace, void* stream);
 
+/* The decoder step's kernels, launched as sb_decoder_step launches them (R hypothesis rows, DEVICE pointers).
+ *
+ * Embedding: x fp32 [R, D] = embed[tokens[r]] * scale + pos_row (bf16 [vocab, D], fp32 [D] = the position's row of the
+ * table, D a multiple of 8); an id outside [0, vocab) sets *err_flag (int32) to 1 and embeds row 0. */
+int sb_decoder_embed(const int64_t* tokens, const void* embed, int64_t vocab, const float* pos_row, int32_t D, float scale,
+                     float* x, int32_t R, int32_t* err_flag, void* stream);
+/* Cached causal self-attention at position t of one layer, D = 64 * H a multiple of 256:
+ *   qkv bf16 [R, 3D] (q | k | v of position t); kcache / vcache bf16 [R, Tmax, D]; table int32 [R, Tmax]
+ *   (table[r, t'] = the cache row holding position t' < t of hypothesis r).  Writes k and v of row r to cache row r at
+ *   position t, then out bf16 [R, D] = softmax(q . k / 8) . v over positions 0..t.  t in [0, Tmax), Tmax <= 512, R <= 65535. */
+int sb_decoder_attention(const void* qkv, void* kcache, void* vcache, const int32_t* table, int32_t t, int32_t R,
+                         int32_t Tmax, int32_t H, void* out, void* stream);
+/* x fp32 [R, D] += c[r / beam] (c fp32 [R / beam, D], one row per sentence); h bf16 [R, D] = LayerNorm(x) * gamma + beta;
+ * D a multiple of 128, at most 1024. */
+int sb_decoder_add_const_layernorm(float* x, const float* c, int32_t R, int32_t beam, int32_t D, const float* gamma,
+                                   const float* beta, float eps, void* h, void* stream);
+/* n-chunks sb_decoder_step splits the vocabulary sweep into for R rows; the head's scratch holds 2 * n_chunks lists. */
+int sb_decoder_vocab_chunks(int32_t R, int64_t V, int32_t* n_chunks);
+/* The vocabulary head: logits = h . embed^T (h bf16 [R, D], embed bf16 [V, D], never materialised) ->
+ *   out_lprob fp32 / out_tok int32 [R, 16]: the 16 best (logit - logsumexp, token), ordered by (value desc, token asc);
+ *   when V < 16 the last 16 - V entries are (-inf, -1);
+ *   out_eos fp32 [R] = log P(eos_idx); probe_tokens int64 [R] or NULL, with it out_probe fp32 [R] = log P(probe_tokens[r])
+ *   (an id outside [0, V) scores token 0).
+ * Caller-owned scratch with L = 2 * n_chunks lists: cand_val fp32 / cand_idx int32 [R, L, 16], lse_part fp32 [R, L, 2].
+ * n_chunks = 0 takes the step's own split (sb_decoder_vocab_chunks); a positive count is used as given, and refused if
+ * some chunk would get no 256-column tile or L > 256. */
+int sb_decoder_vocab_head(const void* h, const void* embed, int32_t R, int64_t V, int32_t D, int32_t eos_idx,
+                          const int64_t* probe_tokens, int32_t n_chunks, float* cand_val, int32_t* cand_idx, float* lse_part,
+                          float* out_lprob, int32_t* out_tok, float* out_eos, float* out_probe, void* stream);
+
 /* ---- speech feature frontend (BASELINE.json config 3, rows a9/a10) ----
  * Replaces fairseq2n WaveformToFbankConverter(num_mel_bins=80, waveform_scale=2**15, channel_last=True,
  * standardize=True) + Collater(pad_value=0, pad_to_multiple=2) (sonar/inference_pipelines/speech.py:120-127,139,

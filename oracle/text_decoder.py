@@ -80,6 +80,13 @@ def make_synthetic_decoder_state_dict(cfg: OracleDecoderConfig, seed: int = 2, w
     return sd
 
 
+def attention_core(q: Tensor, k: Tensor, v: Tensor, mask: Optional[Tensor]) -> Tensor:
+    """softmax(q . k / sqrt(head_dim) + mask) . v of q [B, H, S, hd], k / v [B, H, T, hd] -> [B, S, H * hd]."""
+    b, h, s, hd = q.shape
+    a = F.scaled_dot_product_attention(q, k, v, attn_mask=mask)
+    return a.transpose(1, 2).reshape(b, s, h * hd)
+
+
 class OracleTextDecoder:
     """Teacher-forced full-sequence forward of the decoder (causal self-attention), fp32/fp64 on CPU."""
 
@@ -97,9 +104,7 @@ class OracleTextDecoder:
         q = F.linear(q_in, sd[p + "q_proj.weight"], sd[p + "q_proj.bias"]).view(b, s, h, hd).transpose(1, 2)
         k = F.linear(kv_in, sd[p + "k_proj.weight"], sd[p + "k_proj.bias"]).view(b, t, h, hd).transpose(1, 2)
         v = F.linear(kv_in, sd[p + "v_proj.weight"], sd[p + "v_proj.bias"]).view(b, t, h, hd).transpose(1, 2)
-        a = F.scaled_dot_product_attention(q, k, v, attn_mask=mask)
-        a = a.transpose(1, 2).reshape(b, s, d)
-        return F.linear(a, sd[p + "output_proj.weight"], sd[p + "output_proj.bias"])
+        return F.linear(attention_core(q, k, v, mask), sd[p + "output_proj.weight"], sd[p + "output_proj.bias"])
 
     @torch.no_grad()
     def hidden(self, tokens: Tensor, encoder_output: Tensor) -> Tensor:

@@ -150,6 +150,14 @@ _SIGNATURES = {
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                   C.c_void_p]),
     "sb_decoder_check_inputs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_decoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_int32,
+                                   C.c_void_p, C.c_void_p]),
+    "sb_decoder_attention": (C.c_int, [C.c_void_p] * 4 + [C.c_int32] * 4 + [C.c_void_p] * 2),
+    "sb_decoder_add_const_layernorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                                 C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),
+    "sb_decoder_vocab_chunks": (C.c_int, [C.c_int32, C.c_int64, C.POINTER(C.c_int32)]),
+    "sb_decoder_vocab_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_void_p,
+                                        C.c_int32] + [C.c_void_p] * 8),
     "sb_fbank_tables_bytes": (C.c_size_t, []),
     "sb_fbank_build_tables": (C.c_int, [C.c_void_p]),
     "sb_fbank": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,

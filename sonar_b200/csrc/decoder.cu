@@ -297,6 +297,60 @@ vocab_merge_kernel(const float* __restrict__ cand_val, const int* __restrict__ c
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// launches: sb_decoder_step and the kernel-level entry points below call the same functions
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+// x [R, D] fp32 = E[tokens] * scale + pos_row; ids outside [0, vocab) set *err_flag and embed row 0
+int decoder_embed(const int64_t* tokens, const __nv_bfloat16* embed, long long vocab, const float* pos_row, int D, float scale,
+                  float* x, int R, int* err_flag, cudaStream_t stream) {
+  decode_embed_kernel<<<(unsigned)((R + 7) / 8), 256, 0, stream>>>(tokens, embed, vocab, pos_row, D, scale, x, R, err_flag);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return SB_OK;
+}
+
+// The limits of decode_attention_kernel, with the caller's name in the message: one CTA row per hypothesis (grid y),
+// positions up to the position table, heads in 256-column groups of the residual stream.
+int check_decoder_attention(const char* who, int t, int Tmax, int R, int H) {
+  if (t < 0 || t >= Tmax) { set_last_error("%s: position %d outside [0,%d)", who, t, Tmax); return SB_ERR_INVALID; }
+  if (Tmax > kMaxDecodeLen) { set_last_error("%s: max_len %d > %d", who, Tmax, kMaxDecodeLen); return SB_ERR_INVALID; }
+  if (R <= 0 || R > 65535) { set_last_error("%s: too many rows (%d)", who, R); return SB_ERR_INVALID; }
+  if (H <= 0 || (64 * H) % 256 != 0) { set_last_error("%s: model_dim 64 * %d is not a multiple of 256", who, H); return SB_ERR_INVALID; }
+  return SB_OK;
+}
+
+// qkv bf16 [R, 3D]; caches bf16 [R, Tmax, D] of one layer; table int32 [R, Tmax]; out bf16 [R, D]
+int decoder_attention(const __nv_bfloat16* qkv, __nv_bfloat16* kcache, __nv_bfloat16* vcache, const int32_t* table, int t,
+                      int R, int Tmax, int H, __nv_bfloat16* out, cudaStream_t stream) {
+  decode_attention_kernel<<<dim3((unsigned)((H + 3) / 4), (unsigned)R), 128, 0, stream>>>(qkv, kcache, vcache, table, t, Tmax,
+                                                                                        H, out);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return SB_OK;
+}
+
+// x [R, D] fp32 += c[r / beam]; h [R, D] bf16 = LayerNorm(x)
+int decoder_add_const_layernorm(float* x, const float* c, int R, int beam, int D, const float* gamma, const float* beta,
+                                float eps, __nv_bfloat16* h, cudaStream_t stream) {
+  add_const_layernorm_kernel<<<(unsigned)((R + 7) / 8), 256, 0, stream>>>(x, c, R, beam, D, gamma, beta, eps, h);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return SB_OK;
+}
+
+// The vocabulary head: the top-k sweep of h [R, D] . embed [V, D]^T over n_chunks column chunks into the scratch
+// (cand_val / cand_idx [R, lists, 16], lse_part [R, lists, 2], lists = gemm_topk_lists(n_chunks) <= 256), then the merge.
+int decoder_vocab_head(const __nv_bfloat16* h, const __nv_bfloat16* embed, int R, int V, int D, int eos_idx,
+                       const int64_t* probe_tokens, int n_chunks, float* cand_val, int* cand_idx, float* lse_part,
+                       float* out_lprob, int* out_tok, float* out_eos, float* out_probe, int num_sms, cudaStream_t stream) {
+  if (int rc = gemm_bf16_topk(h, D, embed, D, R, V, D, cand_val, cand_idx, lse_part, n_chunks, 2, num_sms, stream)) return rc;
+  vocab_merge_kernel<kTopkCandidates><<<(unsigned)((R + 7) / 8), 256, 0, stream>>>(
+      cand_val, cand_idx, lse_part, gemm_topk_lists(n_chunks), h, embed, D, eos_idx, R, out_lprob, out_tok, out_eos,
+      probe_tokens, (long long)V, out_probe);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return SB_OK;
+}
+
+}  // namespace
 }  // namespace sb
 
 using namespace sb;
@@ -468,17 +522,14 @@ int sb_decoder_step(SbDecoder* d, const int64_t* tokens, const int32_t* table, i
     set_last_error("sb_decoder_step: probe_tokens and out_probe_lprob go together");
     return SB_ERR_INVALID;
   }
-  if (t < 0 || t >= max_len) { set_last_error("sb_decoder_step: position %d outside [0,%d)", t, max_len); return SB_ERR_INVALID; }
-  if (max_len > kMaxDecodeLen) { set_last_error("sb_decoder_step: max_len %d > %d", max_len, kMaxDecodeLen); return SB_ERR_INVALID; }
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   const int D = d->cfg.model_dim, F = d->cfg.ffn_inner_dim, H = d->cfg.num_heads;
   const int R = N * beam;
-  if (R > 65535) { set_last_error("sb_decoder_step: too many rows (%d)", R); return SB_ERR_INVALID; }
-  const unsigned row_blocks = (unsigned)((R + 7) / 8);
-  decode_embed_kernel<<<row_blocks, 256, 0, stream>>>(tokens, reinterpret_cast<const __nv_bfloat16*>(d->embed),
-                                                      d->cfg.vocab_size, d->pos_table + (size_t)t * D, D,
-                                                      d->cfg.embed_scale, w.x, R, w.err_flag);
-  SB_CUDA_CHECK(cudaGetLastError());
+  if ((rc = check_decoder_attention("sb_decoder_step", t, max_len, R, H))) return rc;
+  const __nv_bfloat16* embed = reinterpret_cast<const __nv_bfloat16*>(d->embed);
+  if ((rc = decoder_embed(tokens, embed, d->cfg.vocab_size, d->pos_table + (size_t)t * D, D, d->cfg.embed_scale, w.x, R,
+                          w.err_flag, stream)))
+    return rc;
   // Every GEMM of a step may take the weight-streaming path; the residual ones may split K when their tiles leave SM
   // pairs idle (2 560 rows).
   auto gemm = [&](GemmArgs g) {
@@ -492,25 +543,19 @@ int sb_decoder_step(SbDecoder* d, const int64_t* tokens, const int32_t* table, i
     const SbDecoderLayerWeights& L = d->layers[li];
     if ((rc = layernorm_bf16(w.x, L.ln1_g, L.ln1_b, d->cfg.ln_eps, w.h, R, D, stream))) return rc;
     if ((rc = gemm(gemm_args(w.h, D, L.wqkv, D, w.qkv, 3 * D, 0, L.bqkv, R, 3 * D, D, EPI_BIAS, d->num_sms)))) return rc;
-    decode_attention_kernel<<<dim3((unsigned)((H + 3) / 4), (unsigned)R), 128, 0, stream>>>(
-        w.qkv, w.kcache + li * layer_stride, w.vcache + li * layer_stride, table, t, max_len, H, w.h);
-    SB_CUDA_CHECK(cudaGetLastError());
+    if ((rc = decoder_attention(w.qkv, w.kcache + li * layer_stride, w.vcache + li * layer_stride, table, t, R, max_len, H, w.h,
+                                stream)))
+      return rc;
     if ((rc = gemm(gemm_args(w.h, D, L.wo, D, w.x, D, 1, L.bo, R, D, D, EPI_BIAS_RESIDUAL, d->num_sms)))) return rc;
-    add_const_layernorm_kernel<<<row_blocks, 256, 0, stream>>>(w.x, w.cross + (size_t)li * N * D, R, beam, D, L.ln3_g,
-                                                               L.ln3_b, d->cfg.ln_eps, w.h);
-    SB_CUDA_CHECK(cudaGetLastError());
+    if ((rc = decoder_add_const_layernorm(w.x, w.cross + (size_t)li * N * D, R, beam, D, L.ln3_g, L.ln3_b, d->cfg.ln_eps, w.h,
+                                          stream)))
+      return rc;
     if ((rc = gemm(gemm_args(w.h, D, L.w1, D, w.f, F, 0, L.b1, R, F, D, EPI_BIAS_RELU, d->num_sms)))) return rc;
     if ((rc = gemm(gemm_args(w.f, F, L.w2, F, w.x, D, 1, L.b2, R, D, F, EPI_BIAS_RESIDUAL, d->num_sms)))) return rc;
   }
   if ((rc = layernorm_bf16(w.x, d->final_ln_g, d->final_ln_b, d->cfg.ln_eps, w.h, R, D, stream))) return rc;
-  if ((rc = gemm_bf16_topk(w.h, D, reinterpret_cast<const __nv_bfloat16*>(d->embed), D, R, (int)d->cfg.vocab_size, D,
-                           w.cand_val, w.cand_idx, w.lse_part, w.n_chunks, 2, d->num_sms, stream)))
-    return rc;
-  vocab_merge_kernel<kTopkCandidates><<<row_blocks, 256, 0, stream>>>(
-      w.cand_val, w.cand_idx, w.lse_part, gemm_topk_lists(w.n_chunks), w.h, reinterpret_cast<const __nv_bfloat16*>(d->embed), D,
-      d->cfg.eos_idx, R, out_lprob, out_tok, out_eos_lprob, probe_tokens, (long long)d->cfg.vocab_size, out_probe_lprob);
-  SB_CUDA_CHECK(cudaGetLastError());
-  return SB_OK;
+  return decoder_vocab_head(w.h, embed, R, (int)d->cfg.vocab_size, D, d->cfg.eos_idx, probe_tokens, w.n_chunks, w.cand_val,
+                            w.cand_idx, w.lse_part, out_lprob, out_tok, out_eos_lprob, out_probe_lprob, d->num_sms, stream);
 }
 
 int sb_decoder_check_inputs(SbDecoder* d, void* workspace, void* stream_v) {
@@ -524,6 +569,71 @@ int sb_decoder_check_inputs(SbDecoder* d, void* workspace, void* stream_v) {
     return SB_ERR_INPUT;
   }
   return SB_OK;
+}
+
+int sb_decoder_embed(const int64_t* tokens, const void* embed, int64_t vocab, const float* pos_row, int32_t D, float scale,
+                     float* x, int32_t R, int32_t* err_flag, void* stream) {
+  if (!tokens || !embed || !pos_row || !x || !err_flag) { set_last_error("sb_decoder_embed: null argument"); return SB_ERR_INVALID; }
+  if (R <= 0 || vocab <= 0 || D <= 0 || D % 8 != 0) {
+    set_last_error("sb_decoder_embed: bad argument (R %d, vocab %lld, D %d)", R, (long long)vocab, D);
+    return SB_ERR_INVALID;
+  }
+  return decoder_embed(tokens, static_cast<const __nv_bfloat16*>(embed), vocab, pos_row, D, scale, x, R, err_flag,
+                       reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sb_decoder_attention(const void* qkv, void* kcache, void* vcache, const int32_t* table, int32_t t, int32_t R,
+                         int32_t Tmax, int32_t H, void* out, void* stream) {
+  if (!qkv || !kcache || !vcache || !table || !out) { set_last_error("sb_decoder_attention: null argument"); return SB_ERR_INVALID; }
+  if (int rc = check_decoder_attention("sb_decoder_attention", t, Tmax, R, H)) return rc;
+  return decoder_attention(static_cast<const __nv_bfloat16*>(qkv), static_cast<__nv_bfloat16*>(kcache),
+                           static_cast<__nv_bfloat16*>(vcache), table, t, R, Tmax, H, static_cast<__nv_bfloat16*>(out),
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sb_decoder_add_const_layernorm(float* x, const float* c, int32_t R, int32_t beam, int32_t D, const float* gamma,
+                                   const float* beta, float eps, void* h, void* stream) {
+  if (!x || !c || !gamma || !beta || !h) { set_last_error("sb_decoder_add_const_layernorm: null argument"); return SB_ERR_INVALID; }
+  if (R <= 0 || beam <= 0 || D <= 0 || D % 128 != 0 || D > 128 * kMaxVec) {
+    set_last_error("sb_decoder_add_const_layernorm: bad argument (R %d, beam %d, D %d; D a multiple of 128 <= %d)", R, beam, D,
+                   128 * kMaxVec);
+    return SB_ERR_INVALID;
+  }
+  return decoder_add_const_layernorm(x, c, R, beam, D, gamma, beta, eps, static_cast<__nv_bfloat16*>(h),
+                                     reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sb_decoder_vocab_chunks(int32_t R, int64_t V, int32_t* n_chunks) {
+  if (!n_chunks || R <= 0 || V <= 0 || V > INT32_MAX) { set_last_error("sb_decoder_vocab_chunks: bad argument"); return SB_ERR_INVALID; }
+  int sms = 0;
+  if (int rc = require_hopper("sb_decoder_vocab_chunks", &sms)) return rc;
+  *n_chunks = gemm_topk_chunks(R, (int)V, 2, sms);
+  return SB_OK;
+}
+
+int sb_decoder_vocab_head(const void* h, const void* embed, int32_t R, int64_t V, int32_t D, int32_t eos_idx,
+                          const int64_t* probe_tokens, int32_t n_chunks, float* cand_val, int32_t* cand_idx, float* lse_part,
+                          float* out_lprob, int32_t* out_tok, float* out_eos, float* out_probe, void* stream) {
+  if (!h || !embed || !cand_val || !cand_idx || !lse_part || !out_lprob || !out_tok || !out_eos ||
+      (probe_tokens != nullptr) != (out_probe != nullptr)) {
+    set_last_error("sb_decoder_vocab_head: null argument (probe_tokens and out_probe go together)");
+    return SB_ERR_INVALID;
+  }
+  if (R <= 0 || V <= 0 || V > INT32_MAX || D <= 0 || eos_idx < 0 || eos_idx >= V || n_chunks < 0) {
+    set_last_error("sb_decoder_vocab_head: bad argument (R %d, V %lld, D %d, eos %d, n_chunks %d)", R, (long long)V, D, eos_idx,
+                   n_chunks);
+    return SB_ERR_INVALID;
+  }
+  int sms = 0;
+  if (int rc = require_hopper("sb_decoder_vocab_head", &sms)) return rc;
+  if (n_chunks == 0) n_chunks = gemm_topk_chunks(R, (int)V, 2, sms);
+  if (gemm_topk_lists(n_chunks) > 256) {  // the merge kernel's per-lane bitmap covers 128 entries: 256 lists of 16
+    set_last_error("sb_decoder_vocab_head: %d chunks give %d candidate lists (at most 256)", n_chunks, gemm_topk_lists(n_chunks));
+    return SB_ERR_INVALID;
+  }
+  return decoder_vocab_head(static_cast<const __nv_bfloat16*>(h), static_cast<const __nv_bfloat16*>(embed), R, (int)V, D, eos_idx,
+                            probe_tokens, n_chunks, cand_val, cand_idx, lse_part, out_lprob, out_tok, out_eos, out_probe, sms,
+                            reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -107,14 +107,18 @@ struct TileSched {
   }
 };
 
-// insert (v, idx) into a descending list kept in registers; equal values keep the earlier entry first
+// insert (v, idx) into a descending list kept in registers; equal values keep the earlier entry first.  Past the
+// insertion point every entry moves down one place: the displaced entry must not be compared again, or it would pass
+// the entries of its own value behind it and a tie at the list's end would lose its earliest entry.
 template <int KC>
 __device__ __forceinline__ void topk_insert(float (&tv)[KC], int (&ti)[KC], float v, int idx) {
   float cv = v;
   int ci = idx;
+  bool shifting = false;
 #pragma unroll
   for (int p = 0; p < KC; ++p) {
-    const bool gt = cv > tv[p];
+    const bool gt = shifting || cv > tv[p];
+    shifting = gt;
     const float ov = tv[p];
     const int oi = ti[p];
     tv[p] = gt ? cv : ov;

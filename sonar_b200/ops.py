@@ -7,6 +7,7 @@ no CPU implementation behind any of them.
 
 from __future__ import annotations
 
+import ctypes as C
 from typing import Optional
 
 import torch
@@ -270,6 +271,100 @@ def speech_frontend(fbank: Tensor, cu_seqlens: Tensor, gamma: Tensor, beta: Tens
                                         gamma.data_ptr(), beta.data_ptr(), eps, out.data_ptr(), _stream())
     _lib.check(rc, "sb_speech_frontend")
     return out
+
+
+def decoder_embed(tokens: Tensor, embed: Tensor, pos_row: Tensor, scale: float, *, out: Optional[Tensor] = None):
+    """The decoder step's embedding (``sb_decoder_embed``): tokens int64 [R], embed bf16 [V, D], pos_row fp32 [D] ->
+    (x fp32 [R, D] = embed[tokens] * scale + pos_row, flag): flag is True if an id lay outside [0, V) (row 0 embedded)."""
+    _need_cuda(tokens, embed, pos_row, out)
+    assert tokens.dtype == torch.int64 and tokens.is_contiguous() and tokens.dim() == 1
+    assert embed.dtype == torch.bfloat16 and embed.is_contiguous() and pos_row.dtype == torch.float32 and pos_row.is_contiguous()
+    r, (v, d) = tokens.numel(), embed.shape
+    assert pos_row.numel() == d
+    if out is None:
+        out = torch.empty((r, d), dtype=torch.float32, device=tokens.device)
+    assert out.dtype == torch.float32 and out.shape == (r, d) and out.is_contiguous()
+    err = torch.zeros(1, dtype=torch.int32, device=tokens.device)
+    rc = _lib.load().sb_decoder_embed(tokens.data_ptr(), embed.data_ptr(), v, pos_row.data_ptr(), d, scale, out.data_ptr(), r,
+                                      err.data_ptr(), _stream())
+    _lib.check(rc, "sb_decoder_embed")
+    return out, bool(err.item())
+
+
+def decoder_attention(qkv: Tensor, kcache: Tensor, vcache: Tensor, table: Tensor, t: int, num_heads: int, *,
+                      out: Optional[Tensor] = None) -> Tensor:
+    """The decoder step's cached self-attention at position t of one layer (``sb_decoder_attention``): qkv bf16 [R, 3D],
+    kcache / vcache bf16 [R, Tmax, D] (updated in place: row r, position t <- k / v of qkv row r), table int32 [R, Tmax]
+    (table[r, t'] = cache row of position t' < t of hypothesis r) -> bf16 [R, D] = softmax(q . k / 8) . v over 0..t."""
+    _need_cuda(qkv, kcache, vcache, table, out)
+    d = 64 * num_heads
+    r = qkv.shape[0]
+    assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and qkv.shape == (r, 3 * d)
+    tmax = kcache.shape[1]
+    for c in (kcache, vcache):
+        assert c.dtype == torch.bfloat16 and c.is_contiguous() and c.shape == (r, tmax, d)
+    assert table.dtype == torch.int32 and table.is_contiguous() and table.shape == (r, tmax)
+    out = _out_rows(out, r, d, qkv.device)
+    rc = _lib.load().sb_decoder_attention(qkv.data_ptr(), kcache.data_ptr(), vcache.data_ptr(), table.data_ptr(), t, r, tmax,
+                                          num_heads, out.data_ptr(), _stream())
+    _lib.check(rc, "sb_decoder_attention")
+    return out
+
+
+def decoder_add_const_layernorm(x: Tensor, c: Tensor, beam: int, gamma: Tensor, beta: Tensor, eps: float = 1e-5, *,
+                                out: Optional[Tensor] = None) -> Tensor:
+    """The decoder layer's cross-attention residual and FFN LayerNorm (``sb_decoder_add_const_layernorm``): x fp32 [R, D]
+    += c[r // beam] in place (c fp32 [R / beam, D]) -> h bf16 [R, D] = LayerNorm(x) * gamma + beta."""
+    _need_cuda(x, c, gamma, beta, out)
+    r, d = x.shape
+    assert x.dtype == c.dtype == torch.float32 and x.is_contiguous() and c.is_contiguous()
+    assert c.shape == ((r + beam - 1) // beam, d) and gamma.numel() == beta.numel() == d
+    out = _out_rows(out, r, d, x.device)
+    rc = _lib.load().sb_decoder_add_const_layernorm(x.data_ptr(), c.data_ptr(), r, beam, d, gamma.data_ptr(), beta.data_ptr(),
+                                                    eps, out.data_ptr(), _stream())
+    _lib.check(rc, "sb_decoder_add_const_layernorm")
+    return out
+
+
+def decoder_vocab_chunks(rows: int, vocab: int) -> int:
+    """The number of column chunks the decoder step splits a vocabulary sweep of `rows` rows into."""
+    n = C.c_int32()
+    _lib.check(_lib.load().sb_decoder_vocab_chunks(rows, vocab, C.byref(n)), "sb_decoder_vocab_chunks")
+    return n.value
+
+
+def decoder_vocab_head(h: Tensor, embed: Tensor, eos_idx: int, probe_tokens: Optional[Tensor] = None, *, n_chunks: int = 0,
+                       out: Optional[tuple] = None):
+    """The decoder step's vocabulary head (``sb_decoder_vocab_head``): h bf16 [R, D], embed bf16 [V, D] ->
+    (lprob fp32 [R, 16], tok int32 [R, 16], eos fp32 [R], probe fp32 [R] or None): the 16 best log-softmax values of
+    h . embed^T by (value desc, token asc), log P(eos_idx) and log P(probe_tokens[r]).  ``n_chunks`` = 0 is the step's own
+    split of the vocabulary; ``out`` optionally gives the four output tensors."""
+    _need_cuda(h, embed, probe_tokens)
+    assert h.dtype == embed.dtype == torch.bfloat16 and h.is_contiguous() and embed.is_contiguous()
+    (r, d), v = h.shape, embed.shape[0]
+    assert embed.shape[1] == d
+    chunks = n_chunks if n_chunks > 0 else decoder_vocab_chunks(r, v)
+    lists = 2 * chunks
+    cand_val = torch.empty((r, lists, 16), dtype=torch.float32, device=h.device)
+    cand_idx = torch.empty((r, lists, 16), dtype=torch.int32, device=h.device)
+    lse_part = torch.empty((r, lists, 2), dtype=torch.float32, device=h.device)
+    if out is None:
+        out = (torch.empty((r, 16), dtype=torch.float32, device=h.device), torch.empty((r, 16), dtype=torch.int32, device=h.device),
+               torch.empty((r,), dtype=torch.float32, device=h.device),
+               None if probe_tokens is None else torch.empty((r,), dtype=torch.float32, device=h.device))
+    lprob, tok, eos, probe = out
+    _need_cuda(lprob, tok, eos, probe)
+    assert lprob.shape == tok.shape == (r, 16) and eos.shape == (r,) and lprob.is_contiguous() and tok.is_contiguous()
+    assert lprob.dtype == eos.dtype == torch.float32 and tok.dtype == torch.int32
+    assert (probe is None) == (probe_tokens is None)
+    if probe_tokens is not None:
+        assert probe_tokens.dtype == torch.int64 and probe_tokens.shape == (r,) and probe.shape == (r,)
+        assert probe.dtype == torch.float32
+    rc = _lib.load().sb_decoder_vocab_head(h.data_ptr(), embed.data_ptr(), r, v, d, eos_idx, _ptr(probe_tokens), n_chunks,
+                                           cand_val.data_ptr(), cand_idx.data_ptr(), lse_part.data_ptr(), lprob.data_ptr(),
+                                           tok.data_ptr(), eos.data_ptr(), _ptr(probe), _stream())
+    _lib.check(rc, "sb_decoder_vocab_head")
+    return lprob, tok, eos, probe
 
 
 LSTM_TILE_ROWS = 64  # sequences per tile of the LSTM recurrent kernel

@@ -36,8 +36,8 @@ def _emb(n, seed=0):
 
 @pytest.mark.parametrize("n,beam,steps", [(3, 2, 9), (26, 3, 5)])
 def test_teacher_forced_steps_match_oracle(small, cuda_device, n, beam, steps):
-    """6 hypothesis rows take the few-rows schedule (skinny GEMMs with the LayerNorms and the cross-attention constant folded
-    in); 78 rows take the wgmma tiles with the separate LayerNorm / add kernels."""
+    """6 hypothesis rows take the weight-streaming skinny GEMMs, 78 rows the wgmma tiles; both run the separate LayerNorm
+    and add + LayerNorm kernels (the decoder folds no LayerNorm into a GEMM)."""
     oracle, model = small
     emb = _emb(n)
     g = torch.Generator().manual_seed(1)
@@ -84,6 +84,38 @@ def test_beam_reordering_through_the_ancestry_table(small, cuda_device):
     seqs = torch.cat([hist[src, :2], new_tok[:, None]], 1)
     ref = oracle.step_lprobs(seqs, emb[:, None, :].repeat_interleave(beam, 0))
     torch.testing.assert_close(lp.cpu(), torch.gather(ref, 1, tok.cpu().long()), rtol=2e-3, atol=2e-2)
+
+
+def test_reordering_at_every_step_to_position_60(small, cuda_device):
+    """Teacher-forced steps to position 60 (four 16-key passes of the cached attention) with a new random within-sentence
+    reordering of the ancestry table before every step, as beam search makes them: each hypothesis's results equal the
+    oracle's on its own gathered token history."""
+    oracle, model = small
+    n, beam, steps = 2, 3, 61
+    r = n * beam
+    emb = _emb(n, seed=12)
+    g = torch.Generator().manual_seed(13)
+    model.begin(emb.to(cuda_device), beam, steps)
+    table = torch.arange(r, dtype=torch.int32)[:, None].expand(r, steps).contiguous()
+    hist = torch.zeros((r, 0), dtype=torch.int64)
+    enc_rows = emb[:, None, :].repeat_interleave(beam, 0)
+    sentence = torch.arange(r) // beam
+    for t in range(steps):
+        if t > 0:  # new hypothesis j continues old hypothesis src[j] of the same sentence
+            src = sentence * beam + torch.randint(0, beam, (r,), generator=g)
+            table = table[src].contiguous()
+            table[:, t - 1] = src.to(torch.int32)  # src's position t - 1 was written to its own cache row
+            hist = hist[src]
+        tok_in = torch.randint(4, VOCAB, (r,), generator=g)
+        probe = torch.randint(4, VOCAB, (r,), generator=g)
+        hist = torch.cat([hist, tok_in[:, None]], 1)
+        lp, tok, eos_lp, probe_lp = model.step(tok_in.to(cuda_device), table.to(cuda_device), t, probe.to(cuda_device))
+        ref = oracle.step_lprobs(hist, enc_rows)
+        lp, tok = lp.cpu(), tok.cpu().long()
+        torch.testing.assert_close(lp, torch.gather(ref, 1, tok), rtol=2e-3, atol=2e-2)
+        torch.testing.assert_close(eos_lp.cpu(), ref[:, 3], rtol=2e-3, atol=2e-2)
+        torch.testing.assert_close(probe_lp.cpu(), torch.gather(ref, 1, probe[:, None])[:, 0], rtol=2e-3, atol=2e-2)
+        assert bool((tok == ref.argmax(1, keepdim=True)).any(1).all()), t
 
 
 def test_generation_is_near_optimal_and_scores_are_honest(small, cuda_device):
