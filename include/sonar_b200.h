@@ -207,10 +207,18 @@ int sb_layernorm(const float* x, const float* gamma, const float* beta, float ep
 int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t H, int64_t total_tokens, void* out,
                  void* stream);
 
-/* x[cu[b]+t,:] = embed[ids[b,t],:]*scale + pos[t,:] ; err_flag DEVICE int32 (set to 1 on a bad id) */
+/* y32 fp32 [T,D] and / or y16 bf16 [T,D] = LayerNorm(x[T,D] fp32), either output may be NULL; y32 may alias x (the
+ * in-place final / pooler LayerNorm of the attention pooling path).  D a multiple of 128, <= 1024. */
+int sb_layernorm_dual(const float* x, const float* gamma, const float* beta, float eps, float* y32, void* y16, int64_t T,
+                      int32_t D, void* stream);
+
+/* x[cu[b]+t,:] = embed[ids[b,t],:]*scale + pos[t,:] for t < min(len_b, S) (ids past a sentence's length are not read);
+ * err_flag DEVICE int32 (set to 1 on an id outside [0, vocab); that row embeds id 0).  h_out / stats_out (both or
+ * neither, D % 256 == 0): the LnFold outputs the encoder's first LayerNorm-consuming GEMM reads -- h_out bf16 [T, D] =
+ * bf16(x), stats_out fp32 [T, D/128, 2] = (mean, M2) of each 128-column chunk of the row of x. */
 int sb_embed(const int64_t* ids, int64_t ids_row_stride, const int32_t* cu_seqlens, int32_t B, int32_t S,
              const void* embed, int64_t vocab, const float* pos_table, int32_t pos_rows, int32_t D, float scale,
-             float* x, int32_t* err_flag, void* stream);
+             float* x, int32_t* err_flag, void* h_out, float* stats_out, void* stream);
 
 /* (optional LayerNorm +) pooling of packed rows x fp32 [T,D] -> out fp32 [B,D] */
 int sb_pool(const float* x, const int32_t* cu_seqlens, int32_t B, int32_t D, const float* gamma, const float* beta,

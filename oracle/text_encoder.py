@@ -135,6 +135,17 @@ def static_pooling(seqs: Tensor, seq_lens: Optional[Tensor], pooling: str) -> Te
     raise NotImplementedError(pooling)
 
 
+def self_attention(q: Tensor, k: Tensor, v: Tensor, key_ok: Optional[Tensor]) -> Tensor:
+    """The encoder layer's attention core (``F.scaled_dot_product_attention`` with a key-padding mask, scale
+    1/sqrt(head_dim)): q, k, v [B, H, S, head_dim], key_ok bool [B, S] (True = a real token) or None (no padding)."""
+    attn_mask = None
+    if key_ok is not None:
+        b, s = key_ok.shape
+        attn_mask = torch.zeros(b, 1, 1, s, dtype=q.dtype, device=q.device)
+        attn_mask.masked_fill_(~key_ok[:, None, None, :], -torch.inf)
+    return F.scaled_dot_product_attention(q, k, v, attn_mask=attn_mask)
+
+
 class OracleTextEncoder:
     """fp32 (or fp64) CPU restatement of ``SonarTextTransformerEncoderModel.forward``
     (``model.py:130-143``) for the ``basic`` wiring (pre-LN layers, no LN inside the
@@ -158,11 +169,7 @@ class OracleTextEncoder:
         # frontend (factory.py:73-100): embed * sqrt(d) + sinusoid, fp32 add then cast [fs2]
         x = F.embedding(ids, sd["encoder_frontend.embed.weight"]) * math.sqrt(d)
         x = (x.float() + self.pos[:s][None]).to(self.dtype)
-        attn_mask = None
-        if seq_lens is not None:
-            key_ok = torch.arange(s)[None, :] < seq_lens[:, None]  # [B,S]
-            attn_mask = torch.zeros(b, 1, 1, s, dtype=self.dtype)
-            attn_mask.masked_fill_(~key_ok[:, None, None, :], -torch.inf)
+        key_ok = None if seq_lens is None else torch.arange(s)[None, :] < seq_lens[:, None]  # [B,S]
         layers = []
         for i in range(cfg.num_layers):
             p = f"encoder.layers.{i}."
@@ -175,7 +182,7 @@ class OracleTextEncoder:
             q = q.view(b, s, h, hd).transpose(1, 2)
             k = k.view(b, s, h, hd).transpose(1, 2)
             v = v.view(b, s, h, hd).transpose(1, 2)
-            a = F.scaled_dot_product_attention(q, k, v, attn_mask=attn_mask)
+            a = self_attention(q, k, v, key_ok)
             a = a.transpose(1, 2).reshape(b, s, d)
             x = r + F.linear(a, sd[p + "self_attn.output_proj.weight"],
                              sd[p + "self_attn.output_proj.bias"])

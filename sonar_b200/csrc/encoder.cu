@@ -131,7 +131,7 @@ static Workspace carve(const SbEncoder* e, int32_t max_batch, int64_t max_tokens
 extern "C" {
 
 const char* sb_last_error(void) { return g_err; }
-int sb_version(void) { return 110; }
+int sb_version(void) { return 111; }
 
 int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbEncoder** out) {
   if (!cfg || !w || !out) { set_last_error("sb_encoder_create: null argument"); return SB_ERR_INVALID; }
@@ -495,6 +495,13 @@ int sb_layernorm(const float* x, const float* gamma, const float* beta, float ep
                         reinterpret_cast<cudaStream_t>(stream));
 }
 
+int sb_layernorm_dual(const float* x, const float* gamma, const float* beta, float eps, float* y32, void* y16, int64_t T,
+                      int32_t D, void* stream) {
+  if (!x || !gamma || !beta || (!y32 && !y16)) { set_last_error("sb_layernorm_dual: null pointer"); return SB_ERR_INVALID; }
+  return layernorm_dual(x, gamma, beta, eps, y32, reinterpret_cast<__nv_bfloat16*>(y16), T, D,
+                        reinterpret_cast<cudaStream_t>(stream));
+}
+
 int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t H, int64_t total_tokens, void* out,
                  void* stream) {
   if (!qkv || !cu_seqlens || !out) { set_last_error("sb_attention: null pointer"); return SB_ERR_INVALID; }
@@ -506,13 +513,14 @@ int sb_attention(const void* qkv, const int32_t* cu_seqlens, int32_t B, int32_t 
 
 int sb_embed(const int64_t* ids, int64_t ids_row_stride, const int32_t* cu_seqlens, int32_t B, int32_t S,
              const void* embed, int64_t vocab, const float* pos_table, int32_t pos_rows, int32_t D, float scale,
-             float* x, int32_t* err_flag, void* stream) {
+             float* x, int32_t* err_flag, void* h_out, float* stats_out, void* stream) {
   if (!ids || !cu_seqlens || !embed || !pos_table || !x || !err_flag) {
     set_last_error("sb_embed: null pointer");
     return SB_ERR_INVALID;
   }
   return embed_tokens(ids, ids_row_stride, cu_seqlens, B, S, reinterpret_cast<const __nv_bfloat16*>(embed), vocab,
-                      pos_table, pos_rows, D, scale, x, err_flag, reinterpret_cast<cudaStream_t>(stream));
+                      pos_table, pos_rows, D, scale, x, err_flag, reinterpret_cast<cudaStream_t>(stream), 0,
+                      reinterpret_cast<__nv_bfloat16*>(h_out), stats_out);
 }
 
 int sb_pool_latent_attention(const void* qt, const void* mem, const int32_t* cu_seqlens, int32_t B, int32_t Hd, int32_t D,

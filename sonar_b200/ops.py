@@ -33,6 +33,13 @@ def _ptr(t: Optional[Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def _out_rows(out: Optional[Tensor], t: int, d: int, device) -> Tensor:
+    if out is None:
+        return torch.empty((t, d), dtype=torch.bfloat16, device=device)
+    assert out.dtype == torch.bfloat16 and out.shape == (t, d) and out.is_contiguous()
+    return out
+
+
 def gemm_bf16(a: Tensor, w: Tensor, bias: Tensor, *, epilogue: str = "bias", residual: Optional[Tensor] = None,
               out_dtype: torch.dtype = torch.bfloat16, out: Optional[Tensor] = None, cta_group: int = 2) -> Tensor:
     """out[M,N] = epi(a[M,K] @ w[N,K]^T + bias[N]); epilogue in {bias, relu, silu, tanh, residual}."""
@@ -66,6 +73,24 @@ def layernorm(x: Tensor, gamma: Tensor, beta: Tensor, eps: float = 1e-5) -> Tens
                                   x.shape[0], x.shape[1], _stream())
     _lib.check(rc, "sb_layernorm")
     return y
+
+
+def layernorm_dual(x: Tensor, gamma: Tensor, beta: Tensor, eps: float = 1e-5, *, out32: Optional[Tensor] = None,
+                   out16: Optional[Tensor] = None):
+    """LayerNorm(x fp32 [T,D]) as fp32 and bf16 rows (``sb_layernorm_dual``, the in-place LayerNorm of the attention
+    pooling path) -> (y32, y16).  ``out32`` may be ``x`` itself."""
+    _need_cuda(x, gamma, beta, out32, out16)
+    assert x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 2
+    t, d = x.shape
+    assert gamma.dtype == beta.dtype == torch.float32 and gamma.numel() == beta.numel() == d
+    if out32 is None:
+        out32 = torch.empty((t, d), dtype=torch.float32, device=x.device)
+    assert out32.dtype == torch.float32 and out32.shape == (t, d) and out32.is_contiguous()
+    out16 = _out_rows(out16, t, d, x.device)
+    rc = _lib.load().sb_layernorm_dual(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), eps, out32.data_ptr(),
+                                       out16.data_ptr(), t, d, _stream())
+    _lib.check(rc, "sb_layernorm_dual")
+    return out32, out16
 
 
 def cu_seqlens_of(seq_lens) -> Tensor:
@@ -132,35 +157,46 @@ def gemm_ln_consumer(a: Tensor, wf: Tensor, bias_f: Tensor, colsum: Tensor, stat
     return out
 
 
-def attention(qkv: Tensor, cu_seqlens: Tensor, num_heads: int) -> Tensor:
+def attention(qkv: Tensor, cu_seqlens: Tensor, num_heads: int, *, out: Optional[Tensor] = None) -> Tensor:
     """Packed bidirectional MHA: qkv bf16 [T, 3*64*H] -> bf16 [T, 64*H]."""
-    _need_cuda(qkv, cu_seqlens)
+    _need_cuda(qkv, cu_seqlens, out)
     assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and cu_seqlens.dtype == torch.int32
     t = qkv.shape[0]
     d = 64 * num_heads
     assert qkv.shape[1] == 3 * d
-    out = torch.empty((t, d), dtype=torch.bfloat16, device=qkv.device)
+    out = _out_rows(out, t, d, qkv.device)
     rc = _lib.load().sb_attention(qkv.data_ptr(), cu_seqlens.data_ptr(), cu_seqlens.numel() - 1, num_heads, t,
                                   out.data_ptr(), _stream())
     _lib.check(rc, "sb_attention")
     return out
 
 
-def embed(ids: Tensor, cu_seqlens: Tensor, table: Tensor, pos_table: Tensor, scale: float, total_tokens: int) -> Tensor:
-    """x[cu[b]+t] = table[ids[b,t]] * scale + pos_table[t]  (fp32 [T, D])."""
-    _need_cuda(ids, cu_seqlens, table, pos_table)
+def embed(ids: Tensor, cu_seqlens: Tensor, table: Tensor, pos_table: Tensor, scale: float, total_tokens: int, *,
+          lnfold: bool = False, out: Optional[Tensor] = None, flag: Optional[Tensor] = None):
+    """x[cu[b]+t] = table[ids[b,t]] * scale + pos_table[t]  (fp32 [T, D]).  With ``lnfold`` -> (x, h, stats): also the
+    LnFold outputs h = bf16(x) [T, D] and stats fp32 [T, D/128, 2], the (mean, M2) of each 128-column chunk of a row.
+    An id outside [0, vocab) raises ValueError, unless ``flag`` (int32 device tensor) is given: the kernel then sets
+    flag[0] to 1 and embeds row 0 for that id."""
+    _need_cuda(ids, cu_seqlens, table, pos_table, out, flag)
     assert ids.dtype == torch.int64 and ids.stride(1) == 1 and table.dtype == torch.bfloat16
     b, s = ids.shape
     d = table.shape[1]
-    x = torch.empty((total_tokens, d), dtype=torch.float32, device=ids.device)
-    err = torch.zeros(1, dtype=torch.int32, device=ids.device)
+    if out is None:
+        out = torch.empty((total_tokens, d), dtype=torch.float32, device=ids.device)
+    assert out.dtype == torch.float32 and out.shape == (total_tokens, d) and out.is_contiguous()
+    h = stats = None
+    if lnfold:
+        h = torch.empty((total_tokens, d), dtype=torch.bfloat16, device=ids.device)
+        stats = torch.empty((total_tokens, d // 128, 2), dtype=torch.float32, device=ids.device)
+    err = torch.zeros(1, dtype=torch.int32, device=ids.device) if flag is None else flag
+    assert err.dtype == torch.int32
     rc = _lib.load().sb_embed(ids.data_ptr(), ids.stride(0), cu_seqlens.data_ptr(), b, s, table.data_ptr(),
-                              table.shape[0], pos_table.data_ptr(), pos_table.shape[0], d, scale, x.data_ptr(),
-                              err.data_ptr(), _stream())
+                              table.shape[0], pos_table.data_ptr(), pos_table.shape[0], d, scale, out.data_ptr(),
+                              err.data_ptr(), _ptr(h), _ptr(stats), _stream())
     _lib.check(rc, "sb_embed")
-    if int(err.item()) != 0:
+    if flag is None and int(err.item()) != 0:
         raise ValueError("sb_embed: token id outside [0, vocab_size)")
-    return x
+    return (out, h, stats) if lnfold else out
 
 
 def pool_packed(x: Tensor, cu_seqlens: Tensor, pooling: str, *, gamma: Optional[Tensor] = None,
@@ -180,16 +216,17 @@ def pool_packed(x: Tensor, cu_seqlens: Tensor, pooling: str, *, gamma: Optional[
     return (out, enc) if enc is not None else out
 
 
-def pool_latent_attention(qt: Tensor, mem: Tensor, cu_seqlens: Tensor) -> Tensor:
+def pool_latent_attention(qt: Tensor, mem: Tensor, cu_seqlens: Tensor, *, out: Optional[Tensor] = None) -> Tensor:
     """The attention pooler's cross-attention on the absorbed form: qt bf16 [B, Hd, D] (Hd <= 16 queries per sentence),
     mem bf16 [T, D] packed rows, cu_seqlens int32 [B+1] -> u bf16 [B, Hd, D] with
     u[b, h] = softmax_t(qt[b, h] . mem[t] / 8) . mem over the rows of sentence b (zeros for an empty sentence)."""
-    _need_cuda(qt, mem, cu_seqlens)
+    _need_cuda(qt, mem, cu_seqlens, out)
     assert qt.dtype == torch.bfloat16 and mem.dtype == torch.bfloat16 and cu_seqlens.dtype == torch.int32
     assert qt.is_contiguous() and mem.is_contiguous() and qt.dim() == 3 and mem.dim() == 2
     b, hd, d = qt.shape
     assert mem.shape[1] == d and cu_seqlens.numel() == b + 1
-    u = torch.empty_like(qt)
+    u = torch.empty_like(qt) if out is None else out
+    assert u.dtype == torch.bfloat16 and u.shape == qt.shape and u.is_contiguous()
     rc = _lib.load().sb_pool_latent_attention(qt.data_ptr(), mem.data_ptr(), cu_seqlens.data_ptr(), b, hd, d,
                                               u.data_ptr(), _stream())
     _lib.check(rc, "sb_pool_latent_attention")
@@ -197,13 +234,6 @@ def pool_latent_attention(qt: Tensor, mem: Tensor, cu_seqlens: Tensor) -> Tensor
 
 
 RELPOS_IMPLS = {"wgmma": 0, "mma_sync": 1}
-
-
-def _out_rows(out: Optional[Tensor], t: int, d: int, device) -> Tensor:
-    if out is None:
-        return torch.empty((t, d), dtype=torch.bfloat16, device=device)
-    assert out.dtype == torch.bfloat16 and out.shape == (t, d) and out.is_contiguous()
-    return out
 
 
 def attention_relpos(qkv: Tensor, p: Tensor, u_bias: Tensor, v_bias: Tensor, cu_seqlens: Tensor, num_heads: int, *,
