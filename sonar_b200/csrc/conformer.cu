@@ -618,11 +618,7 @@ int sb_speech_encoder_create(const SbSpeechConfig* cfg, const SbSpeechWeights* w
   return SB_OK;
 }
 
-void sb_speech_encoder_destroy(SbSpeechEncoder* e) {
-  if (!e) return;
-  e->pooler.destroy();
-  delete e;
-}
+void sb_speech_encoder_destroy(SbSpeechEncoder* e) { delete e; }
 
 int sb_speech_encoder_workspace_bytes(const SbSpeechEncoder* e, int32_t B, int64_t total_positions, int32_t max_positions,
                                       size_t* bytes) {

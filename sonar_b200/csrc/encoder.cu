@@ -32,6 +32,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -63,6 +64,84 @@ int require_hopper(const char* who, int* num_sms) {
   return SB_OK;
 }
 
+StagingRing::~StagingRing() {
+  for (int i = 0; i < num_ev; ++i) cudaEventDestroy(ev[i]);
+  if (pinned) cudaFreeHost(pinned);
+}
+
+int StagingRing::create(const char* who, size_t slot_ints) {
+  this->slot_ints = slot_ints;
+  if (cudaMallocHost(reinterpret_cast<void**>(&pinned), sizeof(int32_t) * kSlots * slot_ints) != cudaSuccess) {
+    pinned = nullptr;
+    set_last_error("%s: cudaMallocHost failed", who);
+    return SB_ERR_CUDA;
+  }
+  for (; num_ev < kSlots; ++num_ev)
+    if (cudaEventCreateWithFlags(&ev[num_ev], cudaEventDisableTiming) != cudaSuccess) {
+      set_last_error("%s: cudaEventCreate failed", who);
+      return SB_ERR_CUDA;
+    }
+  return SB_OK;
+}
+
+int StagingRing::acquire(int32_t** slot) {
+  const unsigned i = next_slot++ % kSlots;
+  SB_CUDA_CHECK(cudaEventSynchronize(ev[i]));  // before the host writes the slot
+  *slot = pinned + (size_t)i * slot_ints;
+  return SB_OK;
+}
+
+int StagingRing::record(cudaStream_t stream) {
+  SB_CUDA_CHECK(cudaEventRecord(ev[(next_slot - 1) % kSlots], stream));
+  return SB_OK;
+}
+
+int host_cu_seqlens(const char* who, const int32_t* lens, int B, int S, int min_len, int32_t* cu, long long* T) {
+  *T = 0;
+  cu[0] = 0;
+  for (int b = 0; b < B; ++b) {
+    const int len = lens ? lens[b] : S;
+    if (len < min_len || len > S) {
+      set_last_error("%s: seq_lens[%d]=%d outside [%d,%d]", who, b, len, min_len, S);
+      return SB_ERR_INVALID;
+    }
+    if ((*T += len) > 0x7fffffffll) {
+      set_last_error("%s: too many tokens (seq_lens[0..%d] sum to more than 2^31 - 1)", who, b);
+      return SB_ERR_INVALID;
+    }
+    cu[b + 1] = (int32_t)*T;
+  }
+  return SB_OK;
+}
+
+int InputFlag::create(const char* who) {
+  if (cudaMalloc(reinterpret_cast<void**>(&dev), 256) != cudaSuccess || cudaMemset(dev, 0, 256) != cudaSuccess) {
+    set_last_error("%s: cudaMalloc of the input-check flag failed", who);
+    return SB_ERR_CUDA;
+  }
+  return SB_OK;
+}
+
+int InputFlag::check(const char* forward, cudaStream_t stream) {
+  int32_t flag = 0;
+  SB_CUDA_CHECK(cudaMemcpyAsync(&flag, dev, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+  SB_CUDA_CHECK(cudaMemsetAsync(dev, 0, sizeof(int32_t), stream));  // sticky until read: covers every forward since
+  SB_CUDA_CHECK(cudaStreamSynchronize(stream));
+  if (flag != 0) {
+    set_last_error("token id outside [0, vocab_size) in a batch passed to %s since the last check", forward);
+    return SB_ERR_INPUT;
+  }
+  return SB_OK;
+}
+
+int sync_prepared(const char* who, const char* what) {
+  if (cudaDeviceSynchronize() != cudaSuccess) {
+    set_last_error("%s: %s failed: %s", who, what, cudaGetErrorString(cudaGetLastError()));
+    return SB_ERR_CUDA;
+  }
+  return SB_OK;
+}
+
 struct Workspace {
   int32_t* cu;
   float* ln_stats;  // [T, D/128, 2] per-row LayerNorm partials (LnFold)
@@ -91,8 +170,8 @@ struct SbEncoder {
   SbEncoderConfig cfg;
   int out_dim;  // width of `out`: embedding_dim with attention pooling, model_dim otherwise
   std::vector<FoldedLayer> folded;
-  void* fold_pool = nullptr;     // one allocation behind all FoldedLayer pointers
-  int32_t* err_flag = nullptr;   // device: sticky "token id out of range" flag, cleared by sb_encoder_check_inputs
+  WeightPool fold_pool;  // behind all FoldedLayer pointers
+  InputFlag err_flag;    // token id out of range, cleared by sb_encoder_check_inputs
   const void* embed;
   const float* pos_table;
   const float* final_ln_g;
@@ -100,13 +179,8 @@ struct SbEncoder {
   std::vector<SbLayerWeights> layers;
   AttentionPooler pooler;  // attention pooling only
   int num_sms;
-  // pinned staging ring for cu_seqlens
-  static constexpr int kSlots = 8;
   static constexpr int kSlotInts = 32768 + 8;
-  int32_t* pinned = nullptr;
-  cudaEvent_t ev[kSlots];
-  bool ev_ok[kSlots];
-  unsigned next_slot = 0;
+  StagingRing staging;  // cu_seqlens
   // optional in-step timing of the dominant kernel (FFN inner-projection GEMM of the middle layer)
   cudaEvent_t prof_start = nullptr, prof_stop = nullptr;
 };
@@ -183,7 +257,7 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
     }
   int num_sms = 0;
   if (int rc = require_hopper("sb_encoder_create", &num_sms)) return rc;
-  SbEncoder* e = new (std::nothrow) SbEncoder();
+  std::unique_ptr<SbEncoder> e(new (std::nothrow) SbEncoder());
   if (!e) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   e->cfg = *cfg;
   e->embed = w->embed;
@@ -193,25 +267,14 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
   e->layers.assign(w->layers, w->layers + cfg->num_layers);
   e->out_dim = attn_pool ? E : D;
   e->num_sms = cfg->num_sms > 0 ? cfg->num_sms : num_sms;
-  for (int i = 0; i < SbEncoder::kSlots; ++i) e->ev_ok[i] = false;
-  if (cudaMallocHost(reinterpret_cast<void**>(&e->pinned), sizeof(int32_t) * SbEncoder::kSlots * SbEncoder::kSlotInts) !=
-      cudaSuccess) {
-    set_last_error("sb_encoder_create: cudaMallocHost failed");
-    delete e;
-    return SB_ERR_CUDA;
-  }
-  if (cudaMalloc(reinterpret_cast<void**>(&e->err_flag), 256) != cudaSuccess ||
-      cudaMemset(e->err_flag, 0, 256) != cudaSuccess) {
-    set_last_error("sb_encoder_create: cudaMalloc of the input-check flag failed");
-    sb_encoder_destroy(e);
-    return SB_ERR_CUDA;
-  }
+  if (int rc = e->staging.create("sb_encoder_create", SbEncoder::kSlotInts)) return rc;
+  if (int rc = e->err_flag.create("sb_encoder_create")) return rc;
   if (cfg->ln_fold && cfg->num_layers > 0) {
     // LayerNorm folding (LnFold): W' = W diag(gamma), c = row sums of W', b' = b + W beta for the two GEMMs that consume a
     // LayerNorm in every layer; prepared once here (the caller's weights are not modified)
     const size_t D_ = D, F_ = F;
-    auto carve_folded = [&](void* base) {
-      Carver c(base);
+    e->folded.resize(cfg->num_layers);
+    int rc = e->fold_pool.alloc("sb_encoder_create", "LayerNorm-folded weights", [&](Carver& c) {
       for (FoldedLayer& f : e->folded) {
         f.wqkv = c.take<__nv_bfloat16>(3 * D_ * D_ * 2, 256);
         f.w1 = c.take<__nv_bfloat16>(F_ * D_ * 2, 256);
@@ -220,59 +283,29 @@ int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbE
         f.c1 = c.take<float>(F_ * 4, 256);
         f.b1 = c.take<float>(F_ * 4, 256);
       }
-      return c.off;
-    };
-    e->folded.resize(cfg->num_layers);
-    const size_t pool_bytes = carve_folded(nullptr);
-    if (cudaMalloc(&e->fold_pool, pool_bytes) != cudaSuccess) {
-      set_last_error("sb_encoder_create: cudaMalloc of %zu bytes for the LayerNorm-folded weights failed", pool_bytes);
-      sb_encoder_destroy(e);
-      return SB_ERR_CUDA;
-    }
-    carve_folded(e->fold_pool);
+    });
+    if (rc) return rc;
     for (int i = 0; i < cfg->num_layers; ++i) {
       const FoldedLayer& f = e->folded[i];
       const SbLayerWeights& l = e->layers[i];
-      int rc = fold_layernorm_weights(reinterpret_cast<const __nv_bfloat16*>(l.wqkv), l.bqkv, l.ln1_g, l.ln1_b, 3 * D, D,
-                                      f.wqkv, f.cqkv, f.bqkv, nullptr);
+      rc = fold_layernorm_weights(reinterpret_cast<const __nv_bfloat16*>(l.wqkv), l.bqkv, l.ln1_g, l.ln1_b, 3 * D, D,
+                                  f.wqkv, f.cqkv, f.bqkv, nullptr);
       if (!rc)
         rc = fold_layernorm_weights(reinterpret_cast<const __nv_bfloat16*>(l.w1), l.b1, l.ln2_g, l.ln2_b, F, D, f.w1, f.c1,
                                     f.b1, nullptr);
-      if (rc) { sb_encoder_destroy(e); return rc; }
+      if (rc) return rc;
     }
-    if (cudaDeviceSynchronize() != cudaSuccess) {
-      set_last_error("sb_encoder_create: folding the LayerNorm weights failed: %s", cudaGetErrorString(cudaGetLastError()));
-      sb_encoder_destroy(e);
-      return SB_ERR_CUDA;
-    }
+    if ((rc = sync_prepared("sb_encoder_create", "folding the LayerNorm weights"))) return rc;
   }
-  if (attn_pool) {
-    const int rc = e->pooler.create("sb_encoder_create", w->pooler, cfg->pooler_layers, w->pooler_q0, w->proj_w, w->proj_b,
-                                    D, E, cfg->pooler_ffn_inner_dim, cfg->ln_eps, e->num_sms, cfg->cta_group == 1 ? 1 : 2, 0);
-    if (rc) { sb_encoder_destroy(e); return rc; }
-  }
-  for (int i = 0; i < SbEncoder::kSlots; ++i) {
-    if (cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming) != cudaSuccess) {
-      set_last_error("sb_encoder_create: cudaEventCreate failed");
-      sb_encoder_destroy(e);
-      return SB_ERR_CUDA;
-    }
-    e->ev_ok[i] = true;
-  }
-  *out = e;
+  if (attn_pool)
+    if (int rc = e->pooler.create("sb_encoder_create", w->pooler, cfg->pooler_layers, w->pooler_q0, w->proj_w, w->proj_b,
+                                  D, E, cfg->pooler_ffn_inner_dim, cfg->ln_eps, e->num_sms, cfg->cta_group == 1 ? 1 : 2, 0))
+      return rc;
+  *out = e.release();
   return SB_OK;
 }
 
-void sb_encoder_destroy(SbEncoder* e) {
-  if (!e) return;
-  for (int i = 0; i < SbEncoder::kSlots; ++i)
-    if (e->ev_ok[i]) cudaEventDestroy(e->ev[i]);
-  if (e->pinned) cudaFreeHost(e->pinned);
-  if (e->fold_pool) cudaFree(e->fold_pool);
-  e->pooler.destroy();
-  if (e->err_flag) cudaFree(e->err_flag);
-  delete e;
-}
+void sb_encoder_destroy(SbEncoder* e) { delete e; }
 
 int sb_encoder_workspace_bytes(const SbEncoder* enc, int32_t max_batch, int64_t max_tokens, size_t* bytes) {
   if (!enc || !bytes || max_batch <= 0 || max_tokens <= 0) {
@@ -298,24 +331,16 @@ int sb_encoder_forward(SbEncoder* e, const int64_t* ids, int64_t ids_row_stride,
   const int D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, H = e->cfg.num_heads;
 
   // ---- cu_seqlens on the host, staged through a pinned ring ----
-  const unsigned slot = e->next_slot++ % SbEncoder::kSlots;
-  SB_CUDA_CHECK(cudaEventSynchronize(e->ev[slot]));  // only blocks if 8 forwards are still in flight
-  int32_t* cu_h = e->pinned + (size_t)slot * SbEncoder::kSlotInts;
-  long long T = 0;
-  cu_h[0] = 0;
-  for (int b = 0; b < B; ++b) {
-    const int len = seq_lens_host ? seq_lens_host[b] : S;
-    if (len < 0 || len > S) { set_last_error("sb_encoder_forward: seq_lens[%d]=%d outside [0,%d]", b, len, S); return SB_ERR_INVALID; }
-    T += len;
-    if (T > 0x7fffffffll) { set_last_error("sb_encoder_forward: too many tokens"); return SB_ERR_INVALID; }
-    cu_h[b + 1] = (int32_t)T;
-  }
+  int32_t* cu_h;
+  long long T;
+  int rc = e->staging.acquire(&cu_h);
+  if (!rc) rc = host_cu_seqlens("sb_encoder_forward", seq_lens_host, B, S, 0, cu_h, &T);
+  if (rc) return rc;
   Workspace w;
-  int rc = bind_workspace("sb_encoder_forward", workspace, workspace_bytes, &w,
-                          [&](void* p) { return carve(e, B, T, p); });
+  rc = bind_workspace("sb_encoder_forward", workspace, workspace_bytes, &w, [&](void* p) { return carve(e, B, T, p); });
   if (rc) return rc;
   SB_CUDA_CHECK(cudaMemcpyAsync(w.cu, cu_h, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice, stream));
-  SB_CUDA_CHECK(cudaEventRecord(e->ev[slot], stream));
+  if ((rc = e->staging.record(stream))) return rc;
   const bool attn_pool = e->cfg.pooling == SB_POOL_ATTENTION;
   if (T == 0) {
     if (!attn_pool) {
@@ -330,7 +355,7 @@ int sb_encoder_forward(SbEncoder* e, const int64_t* ids, int64_t ids_row_stride,
   const bool fold2 = fold && e->cfg.ln_fold == 1;                   // LN2 (FFN block) folded into out-proj -> FFN1 as well
   __nv_bfloat16* hn = w.qkv;  // [T, D] view of the (dead after attention) qkv buffer: bf16(x) behind the out-projection
   if ((rc = embed_tokens(ids, ids_row_stride, w.cu, B, S, reinterpret_cast<const __nv_bfloat16*>(e->embed),
-                         e->cfg.vocab_size, e->pos_table, e->cfg.pos_rows, D, e->cfg.embed_scale, w.x, e->err_flag,
+                         e->cfg.vocab_size, e->pos_table, e->cfg.pos_rows, D, e->cfg.embed_scale, w.x, e->err_flag.dev,
                          stream, 0, fold ? w.h : nullptr, fold ? w.ln_stats : nullptr)))
     return rc;
 
@@ -418,16 +443,7 @@ int sb_encoder_profile_ffn1(SbEncoder* e, void* start_event, void* stop_event) {
 int sb_encoder_check_inputs(SbEncoder* e, void* workspace, void* stream_v) {
   (void)workspace;  // (kept in the signature; the flag lives in the handle since v101)
   if (!e) { set_last_error("sb_encoder_check_inputs: null argument"); return SB_ERR_INVALID; }
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  int32_t flag = 0;
-  SB_CUDA_CHECK(cudaMemcpyAsync(&flag, e->err_flag, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
-  SB_CUDA_CHECK(cudaMemsetAsync(e->err_flag, 0, sizeof(int32_t), stream));  // sticky until read: covers every forward since
-  SB_CUDA_CHECK(cudaStreamSynchronize(stream));
-  if (flag != 0) {
-    set_last_error("token id outside [0, vocab_size) in a batch passed to sb_encoder_forward since the last check");
-    return SB_ERR_INPUT;
-  }
-  return SB_OK;
+  return e->err_flag.check("sb_encoder_forward", reinterpret_cast<cudaStream_t>(stream_v));
 }
 
 // ---------------------------------------------------------------------------------------------

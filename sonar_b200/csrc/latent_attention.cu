@@ -297,35 +297,18 @@ int AttentionPooler::create(const char* who, const SbPoolerLayerWeights* w, int 
   for (int i = 0; i < num_layers; ++i) layers[i].w = w[i];
   // absorbed cross-attention weights of every layer; the caller's weights are not modified
   const size_t HdD = (size_t)(E / 64) * D, Es = E;
-  auto carve = [&](void* base) {
-    Carver c(base);
+  int rc = absorbed.alloc(who, "absorbed pooler weights", [&](Carver& c) {
     for (Layer& l : layers) {
       l.wqk = c.take<__nv_bfloat16>(HdD * Es * 2, 256);
       l.bqk = c.take<float>(HdD * 4, 256);
       l.wvo = c.take<__nv_bfloat16>(Es * HdD * 2, 256);
       l.bvo = c.take<float>(Es * 4, 256);
     }
-    return c.off;
-  };
-  const size_t bytes = carve(nullptr);
-  if (bytes && cudaMalloc(&absorbed, bytes) != cudaSuccess) {
-    absorbed = nullptr;
-    set_last_error("%s: cudaMalloc of %zu bytes for the absorbed pooler weights failed", who, bytes);
-    return SB_ERR_CUDA;
-  }
-  carve(absorbed);
+  });
+  if (rc) return rc;
   for (const Layer& l : layers)
-    if (int rc = absorb_pooler_weights(l.w, D, E, l.wqk, l.bqk, l.wvo, l.bvo, nullptr)) return rc;
-  if (cudaDeviceSynchronize() != cudaSuccess) {
-    set_last_error("%s: absorbing the pooler weights failed: %s", who, cudaGetErrorString(cudaGetLastError()));
-    return SB_ERR_CUDA;
-  }
-  return SB_OK;
-}
-
-void AttentionPooler::destroy() {
-  if (absorbed) cudaFree(absorbed);
-  absorbed = nullptr;
+    if ((rc = absorb_pooler_weights(l.w, D, E, l.wqk, l.bqk, l.wvo, l.bvo, nullptr))) return rc;
+  return sync_prepared(who, "absorbing the pooler weights");
 }
 
 AttentionPooler::Ws AttentionPooler::take(Carver& c, size_t B) const {

@@ -28,6 +28,7 @@
 #include <math_constants.h>
 
 #include <algorithm>
+#include <memory>
 #include <new>
 #include <numeric>
 #include <vector>
@@ -363,19 +364,15 @@ struct SbLaser2 {
   SbLaser2Config cfg;
   int dirs = 1;
   const void* embed = nullptr;
-  void* packed = nullptr;  // one allocation behind every repacked weight below
+  WeightPool packed;  // behind every repacked weight below
   std::vector<__nv_bfloat16*> w_ih;  // per layer [dirs * 4H, in_l], rows in lstm_gate_row order per direction
   std::vector<float*> bias;          // per layer [dirs * 4H] = b_ih + b_hh, same order
   std::vector<__nv_bfloat16*> w_hh;  // per layer [dirs, 4H, H], same order
-  int32_t* err_flag = nullptr;
+  InputFlag err_flag;
   int num_sms = 0;
   static constexpr int kMaxBatch = 32768;
-  static constexpr int kSlots = 8;
   static constexpr int kSlotInts = (kMaxBatch + 1) + kMaxBatch + kLstmRows;
-  int32_t* pinned = nullptr;
-  cudaEvent_t ev[kSlots];
-  bool ev_ok[kSlots] = {};
-  unsigned next_slot = 0;
+  StagingRing staging;  // cu_seqlens, then the length-sorted tiles
 };
 
 static LaserWs laser_carve(const SbLaser2* e, long long B, long long T, void* base) {
@@ -417,46 +414,29 @@ int sb_laser2_create(const SbLaser2Config* cfg, const SbLaser2Weights* w, SbLase
   int num_sms = 0;
   if (int rc = require_hopper("sb_laser2_create", &num_sms)) return rc;
   if (int rc = lstm_check_cluster_fit("sb_laser2_create")) return rc;
-  SbLaser2* e = new (std::nothrow) SbLaser2();
+  std::unique_ptr<SbLaser2> e(new (std::nothrow) SbLaser2());
   if (!e) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   e->cfg = *cfg;
   e->dirs = dirs;
   e->embed = w->embed;
   e->num_sms = cfg->num_sms > 0 ? cfg->num_sms : num_sms;
-  if (cudaMallocHost(reinterpret_cast<void**>(&e->pinned), sizeof(int32_t) * SbLaser2::kSlots * SbLaser2::kSlotInts) !=
-      cudaSuccess) {
-    set_last_error("sb_laser2_create: cudaMallocHost failed");
-    sb_laser2_destroy(e);
-    return SB_ERR_CUDA;
-  }
-  if (cudaMalloc(reinterpret_cast<void**>(&e->err_flag), 256) != cudaSuccess || cudaMemset(e->err_flag, 0, 256) != cudaSuccess) {
-    set_last_error("sb_laser2_create: cudaMalloc of the input-check flag failed");
-    sb_laser2_destroy(e);
-    return SB_ERR_CUDA;
-  }
+  if (int rc = e->staging.create("sb_laser2_create", SbLaser2::kSlotInts)) return rc;
+  if (int rc = e->err_flag.create("sb_laser2_create")) return rc;
   // repacked weights: W_ih / W_hh rows and the summed bias in the recurrent kernel's gate order (the caller's weights are
   // not modified)
   const size_t G4 = 4 * kLstmH;
   e->w_ih.resize(L);
   e->bias.resize(L);
   e->w_hh.resize(L);
-  auto carve_packed = [&](void* base) {
-    Carver c(base);
+  int rc = e->packed.alloc("sb_laser2_create", "repacked LSTM weights", [&](Carver& c) {
     for (int l = 0; l < L; ++l) {
       const size_t in = l == 0 ? (size_t)cfg->embed_dim : (size_t)dirs * kLstmH;
       e->w_ih[l] = c.take<__nv_bfloat16>(dirs * G4 * in * 2, 256);
       e->bias[l] = c.take<float>(dirs * G4 * 4, 256);
       e->w_hh[l] = c.take<__nv_bfloat16>(dirs * G4 * kLstmH * 2, 256);
     }
-    return c.off;
-  };
-  const size_t packed_bytes = carve_packed(nullptr);
-  if (cudaMalloc(&e->packed, packed_bytes) != cudaSuccess) {
-    set_last_error("sb_laser2_create: cudaMalloc of %zu bytes for the repacked LSTM weights failed", packed_bytes);
-    sb_laser2_destroy(e);
-    return SB_ERR_CUDA;
-  }
-  carve_packed(e->packed);
+  });
+  if (rc) return rc;
   for (int l = 0; l < L; ++l) {
     const int in = l == 0 ? cfg->embed_dim : dirs * kLstmH;
     for (int d = 0; d < dirs; ++d) {
@@ -467,32 +447,12 @@ int sb_laser2_create(const SbLaser2Config* cfg, const SbLaser2Weights* w, SbLase
       lstm_repack_bias_kernel<<<(unsigned)(G4 / 256), 256>>>(lw.b_ih, lw.b_hh, e->bias[l] + d * G4);
     }
   }
-  if (cudaDeviceSynchronize() != cudaSuccess) {
-    set_last_error("sb_laser2_create: repacking the LSTM weights failed: %s", cudaGetErrorString(cudaGetLastError()));
-    sb_laser2_destroy(e);
-    return SB_ERR_CUDA;
-  }
-  for (int i = 0; i < SbLaser2::kSlots; ++i) {
-    if (cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming) != cudaSuccess) {
-      set_last_error("sb_laser2_create: cudaEventCreate failed");
-      sb_laser2_destroy(e);
-      return SB_ERR_CUDA;
-    }
-    e->ev_ok[i] = true;
-  }
-  *out = e;
+  if ((rc = sync_prepared("sb_laser2_create", "repacking the LSTM weights"))) return rc;
+  *out = e.release();
   return SB_OK;
 }
 
-void sb_laser2_destroy(SbLaser2* e) {
-  if (!e) return;
-  for (int i = 0; i < SbLaser2::kSlots; ++i)
-    if (e->ev_ok[i]) cudaEventDestroy(e->ev[i]);
-  if (e->pinned) cudaFreeHost(e->pinned);
-  if (e->packed) cudaFree(e->packed);
-  if (e->err_flag) cudaFree(e->err_flag);
-  delete e;
-}
+void sb_laser2_destroy(SbLaser2* e) { delete e; }
 
 int sb_laser2_workspace_bytes(const SbLaser2* e, int32_t max_batch, int64_t max_tokens, size_t* bytes) {
   if (!e || !bytes || max_batch <= 0 || max_tokens <= 0) {
@@ -515,40 +475,30 @@ int sb_laser2_forward(SbLaser2* e, const int64_t* ids, int64_t ids_row_stride, c
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   const int dirs = e->dirs, H = kLstmH, tiles = lstm_tiles(B);
 
-  // cu_seqlens and the length-sorted tiles on the host, staged through a pinned ring
-  const unsigned slot = e->next_slot++ % SbLaser2::kSlots;
-  SB_CUDA_CHECK(cudaEventSynchronize(e->ev[slot]));  // only blocks if 8 forwards are still in flight
-  int32_t* cu_h = e->pinned + (size_t)slot * SbLaser2::kSlotInts;
+  // cu_seqlens (a packed LSTM sequence cannot be empty) and the length-sorted tiles on the host, staged through a pinned ring
+  int32_t* cu_h;
+  long long T;
+  int rc = e->staging.acquire(&cu_h);
+  if (!rc) rc = host_cu_seqlens("sb_laser2_forward", seq_lens_host, B, S, 1, cu_h, &T);
+  if (rc) return rc;
   int32_t* tiles_h = cu_h + (B + 1);
-  long long T = 0;
-  cu_h[0] = 0;
-  for (int b = 0; b < B; ++b) {
-    const int len = seq_lens_host ? seq_lens_host[b] : S;
-    if (len < 1 || len > S) {
-      set_last_error("sb_laser2_forward: seq_lens[%d]=%d outside [1,%d] (a packed LSTM sequence cannot be empty)", b, len, S);
-      return SB_ERR_INVALID;
-    }
-    T += len;
-    if (T > 0x7fffffffll) { set_last_error("sb_laser2_forward: too many tokens"); return SB_ERR_INVALID; }
-    cu_h[b + 1] = (int32_t)T;
-  }
   // longest first, so that a tile runs about as many steps as its rows need; ties keep the input order
   std::iota(tiles_h, tiles_h + B, 0);
   std::stable_sort(tiles_h, tiles_h + B, [&](int x, int y) { return cu_h[x + 1] - cu_h[x] > cu_h[y + 1] - cu_h[y]; });
   std::fill(tiles_h + B, tiles_h + (size_t)tiles * kLstmRows, -1);
 
   LaserWs w;
-  int rc = bind_workspace("sb_laser2_forward", workspace, workspace_bytes, &w, [&](void* p) { return laser_carve(e, B, T, p); });
+  rc = bind_workspace("sb_laser2_forward", workspace, workspace_bytes, &w, [&](void* p) { return laser_carve(e, B, T, p); });
   if (rc) return rc;
   SB_CUDA_CHECK(cudaMemcpyAsync(w.cu, cu_h, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice, stream));
   SB_CUDA_CHECK(cudaMemcpyAsync(w.tile_seqs, tiles_h, sizeof(int32_t) * (size_t)tiles * kLstmRows, cudaMemcpyHostToDevice,
                                 stream));
-  SB_CUDA_CHECK(cudaEventRecord(e->ev[slot], stream));
+  if ((rc = e->staging.record(stream))) return rc;
 
   const int E = e->cfg.embed_dim;
   laser_embed_kernel<<<B, 128, 0, stream>>>(ids, ids_row_stride, w.cu, S, reinterpret_cast<const int4*>(e->embed),
                                             e->cfg.vocab_size, E, e->cfg.pad_idx, reinterpret_cast<int4*>(w.xy), w.pad,
-                                            w.tail, e->err_flag);
+                                            w.tail, e->err_flag.dev);
   SB_CUDA_CHECK(cudaGetLastError());
   const int N = dirs * 4 * H;
   for (int l = 0; l < e->cfg.num_layers; ++l) {
@@ -572,16 +522,7 @@ int sb_laser2_forward(SbLaser2* e, const int64_t* ids, int64_t ids_row_stride, c
 
 int sb_laser2_check_inputs(SbLaser2* e, void* stream_v) {
   if (!e) { set_last_error("sb_laser2_check_inputs: null argument"); return SB_ERR_INVALID; }
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  int32_t flag = 0;
-  SB_CUDA_CHECK(cudaMemcpyAsync(&flag, e->err_flag, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
-  SB_CUDA_CHECK(cudaMemsetAsync(e->err_flag, 0, sizeof(int32_t), stream));
-  SB_CUDA_CHECK(cudaStreamSynchronize(stream));
-  if (flag != 0) {
-    set_last_error("token id outside [0, vocab_size) in a batch passed to sb_laser2_forward since the last check");
-    return SB_ERR_INPUT;
-  }
-  return SB_OK;
+  return e->err_flag.check("sb_laser2_forward", reinterpret_cast<cudaStream_t>(stream_v));
 }
 
 int sb_lstm_recurrent(const void* G, int64_t ldg, const void* w_hh, const int32_t* cu_seqlens, const int32_t* tile_seqs,

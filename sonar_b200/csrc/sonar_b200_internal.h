@@ -86,6 +86,69 @@ int bind_workspace(const char* who, void* workspace, size_t workspace_bytes, Lay
   return SB_OK;
 }
 
+// ---- what an engine handle owns: each type frees it in its destructor, also after a failed create(), so none is copied ----
+struct NoCopy {
+  NoCopy() = default;
+  NoCopy(const NoCopy&) = delete;
+  NoCopy& operator=(const NoCopy&) = delete;
+};
+
+// Pinned host ring through which a forward stages its per-batch host data (cu_seqlens, ...) for its H2D copies without
+// synchronising with the stream: kSlots slots of `slot_ints` int32, one event per slot.
+struct StagingRing : NoCopy {
+  static constexpr int kSlots = 8;
+  int32_t* pinned = nullptr;
+  size_t slot_ints = 0;
+  cudaEvent_t ev[kSlots];
+  int num_ev = 0;  // ev[0 .. num_ev) exist
+  unsigned next_slot = 0;
+  ~StagingRing();
+  int create(const char* who, size_t slot_ints);  // errors name `who`
+  // *slot = the next slot, once the copies that read it last have completed (this blocks only while kSlots forwards are
+  // in flight).  The caller writes it, enqueues the copies that read it, then calls record().
+  int acquire(int32_t** slot);
+  // The slot acquire() returned stays in use until the work enqueued on `stream` so far has completed.
+  int record(cudaStream_t stream);
+};
+
+// cu[0] = 0, cu[b + 1] = lens[0] + ... + lens[b] for the B host lengths (every one S when lens is null), and *T = cu[B].
+// SB_ERR_INVALID, naming `who` and the offending index, unless each length lies in [min_len, S] and the total fits in int32.
+int host_cu_seqlens(const char* who, const int32_t* lens, int B, int S, int min_len, int32_t* cu, long long* T);
+
+// Device flag (256 bytes, zeroed at create) that an engine's embedding kernel sets on a token id outside the vocabulary.
+// It stays set over any number of forwards until check() reads it.
+struct InputFlag : NoCopy {
+  int32_t* dev = nullptr;
+  ~InputFlag() { cudaFree(dev); }
+  int create(const char* who);
+  // Reads and clears the flag, synchronises `stream`: SB_ERR_INPUT, naming `forward`, if it was set since the last check.
+  int check(const char* forward, cudaStream_t stream);
+};
+
+// One device allocation behind the weights an engine prepares at create (LayerNorm-folded, repacked, absorbed).
+struct WeightPool : NoCopy {
+  void* base = nullptr;
+  ~WeightPool() { cudaFree(base); }
+  // Sizes the pool by running layout(Carver&) on a null base, allocates it (nothing for zero bytes) and runs layout on it,
+  // which sets the caller's pointers.  SB_ERR_CUDA, "<who>: cudaMalloc of N bytes for the <what> failed", on failure.
+  template <class Layout>
+  int alloc(const char* who, const char* what, Layout&& layout) {
+    Carver sizing(nullptr);
+    layout(sizing);
+    if (sizing.off && cudaMalloc(&base, sizing.off) != cudaSuccess) {
+      base = nullptr;
+      set_last_error("%s: cudaMalloc of %zu bytes for the %s failed", who, sizing.off, what);
+      return SB_ERR_CUDA;
+    }
+    Carver c(base);
+    layout(c);
+    return SB_OK;
+  }
+};
+
+// Synchronises after the kernels that prepared an engine's weights: SB_ERR_CUDA, "<who>: <what> failed: <error>", on failure.
+int sync_prepared(const char* who, const char* what);
+
 // cudaFuncSetAttribute is per device: returns true the first time `flags` (a per-call-site static array of 64 bools)
 // is consulted for the current device.
 inline bool first_use_on_device(bool (&flags)[64]) {
@@ -260,7 +323,7 @@ struct AttentionPooler {
     __nv_bfloat16* u = nullptr;   // [B, Hd*D] latent attention output
   };
   std::vector<Layer> layers;
-  void* absorbed = nullptr;  // one device allocation behind every layer's absorbed weights
+  WeightPool absorbed;  // behind every layer's absorbed weights
   const float* q0 = nullptr;      // fp32 [E]
   const void* proj_w = nullptr;   // bf16 [E, E]
   const float* proj_b = nullptr;  // fp32 [E]
@@ -269,11 +332,9 @@ struct AttentionPooler {
   int num_sms = 0, cta_group = 2, allow_skinny = 0;  // GEMM policy
 
   // Checks the weight pointers, copies the layers and absorbs their cross-attention weights into one allocation of
-  // num_layers * (2 Hd D E * 2 + (Hd D + E) * 4) bytes, then synchronises the device.  Errors name `who`; on failure the
-  // caller still calls destroy().
+  // num_layers * (2 Hd D E * 2 + (Hd D + E) * 4) bytes, then synchronises the device.  Errors name `who`.
   int create(const char* who, const SbPoolerLayerWeights* w, int num_layers, const float* q0, const void* proj_w,
              const float* proj_b, int D, int E, int F, float eps, int num_sms, int cta_group, int allow_skinny);
-  void destroy();
   Ws take(Carver& c, size_t B) const;  // the next buffers of a workspace layout, for B sequences
   // out [B, E] fp32 from the memory mem [T, D] bf16 packed by cu_seqlens [B + 1]
   int forward(const Ws& w, const __nv_bfloat16* mem, const int32_t* cu_seqlens, int B, float* out, cudaStream_t stream) const;

@@ -1,7 +1,8 @@
 """The engines' host side: every C-ABI entry point that carves the caller's workspace rejects one that is too small
-(SB_ERR_INVALID, a message that names the entry point) instead of writing past its end, and the Python wrappers keep the
-weights the engines point into out of reach of ``nn.Module`` conversions.  Engines are the small configurations of the
-other GPU tests."""
+(SB_ERR_INVALID, a message that names the entry point) instead of writing past its end, the Python wrappers keep the
+weights the engines point into out of reach of ``nn.Module`` conversions, and the pinned ring through which the text
+encoder and LASER2 stage their host lengths is not rewritten while a copy still reads it.  Engines are the small
+configurations of the other GPU tests."""
 
 import ctypes as C
 
@@ -115,3 +116,62 @@ def test_module_conversions_leave_the_engines_alone(engines, cuda_device):
         after = run()
         torch.cuda.synchronize(cuda_device)
         assert all(torch.equal(a, b) for a, b in zip(before, after)), name
+
+
+@pytest.fixture(scope="module")
+def laser2(native_lib, cuda_device):
+    from oracle.laser_lstm import OracleLaser2Config, make_synthetic_laser2_state_dict
+    from sonar_b200 import B200LaserLstmEncoder, Laser2Config
+
+    cfg = OracleLaser2Config(vocabulary_size=VOCAB, model_dim=128, num_layers=2, bidirectional=True)
+    sd = make_synthetic_laser2_state_dict(cfg, seed=4, weight_bound=0.1)
+    return B200LaserLstmEncoder(Laser2Config(vocabulary_size=VOCAB, pad_idx=cfg.pad_idx, model_dim=cfg.model_dim,
+                                             num_layers=cfg.num_layers, bidirectional=cfg.bidirectional), sd, cuda_device)
+
+
+@pytest.mark.parametrize("engine", ["text_encoder", "laser2"])
+def test_a_burst_that_laps_the_staging_ring(engines, laser2, cuda_device, engine):
+    """17 forwards, more than twice the ring's 8 slots, enqueued on one stream behind a sleeping kernel with no host
+    synchronise, so the host laps the ring while the first forwards still wait: every output is bitwise that of the same
+    batch run on its own.  One out-of-range id in a middle forward makes check_inputs raise once; that check clears it."""
+    from sonar_b200 import PaddingMask, SequenceBatch
+
+    burst, max_batch, S = 17, 48, 40
+    dev = cuda_device
+    if engine == "text_encoder":
+        model = engines[0]
+
+        def run(ids, lens):
+            return model(SequenceBatch(ids, PaddingMask(torch.tensor(lens), S, lens))).sentence_embeddings
+    else:
+        model = laser2
+
+        def run(ids, lens):
+            return model(ids, torch.tensor(lens))
+
+    g = torch.Generator().manual_seed(17)
+    batches = []
+    for _ in range(burst):
+        lens = torch.randint(1, S + 1, (int(torch.randint(1, max_batch + 1, (1,), generator=g)),), generator=g).tolist()
+        ids = torch.ones((len(lens), S), dtype=torch.int64)  # pad_idx 1
+        for i, n in enumerate(lens):
+            ids[i, :n] = torch.randint(4, VOCAB, (n,), generator=g)
+        batches.append((ids.to(dev), lens))  # on the device already: the wrappers make no blocking copy
+    assert len({tuple(lens) for _, lens in batches}) == burst
+    batches[burst // 2][0][0, 0] = VOCAB
+
+    run(torch.full((max_batch, S), 5, dtype=torch.int64, device=dev), [S] * max_batch)  # grows the workspace once
+    torch.cuda.synchronize(dev)
+    model.check_inputs()
+    torch.cuda._sleep(50_000_000)  # tens of milliseconds: the stream is busy while the host enqueues the burst
+    outs = [run(ids, lens) for ids, lens in batches]
+    torch.cuda.synchronize(dev)
+    with pytest.raises(ValueError, match="vocab"):
+        model.check_inputs()
+    model.check_inputs()
+    for i, (ids, lens) in enumerate(batches):
+        alone = run(ids, lens)
+        torch.cuda.synchronize(dev)
+        assert torch.equal(outs[i], alone), f"{engine}: forward {i} of the burst"
+    with pytest.raises(ValueError, match="vocab"):  # set again by the out-of-range batch on its own
+        model.check_inputs()
