@@ -520,7 +520,7 @@ typedef struct SbLstmLayerWeights {
 } SbLstmLayerWeights;
 
 typedef struct SbLaser2Weights {
-  const void* embed;                /* bf16 [vocab, embed_dim]  embed_tokens.weight */
+  const void* embed;                /* bf16 [vocab, embed_dim]  embed_tokens.weight, 16-byte aligned (read as 16-byte rows) */
   const SbLstmLayerWeights* layers; /* HOST array of num_layers * (1 + bidirectional) entries: entry k * dirs + d is layer k,
                                      * direction d (d = 1: the _reverse weights); copied at create */
 } SbLaser2Weights;
@@ -544,18 +544,40 @@ int sb_laser2_forward(SbLaser2* enc, const int64_t* ids, int64_t ids_row_stride,
 /* Checks the sticky device-side flag (token id outside [0, vocab_size)) of the forwards since the last check; synchronises
  * `stream`.  Returns SB_OK or SB_ERR_INPUT. */
 int sb_laser2_check_inputs(SbLaser2* enc, void* stream);
+/* Read-only view of the handle's repacked weights of layer `layer` (DEVICE pointers owned by the handle, valid until
+ * sb_laser2_destroy; rows in the gate order of sb_lstm_recurrent, direction d at rows d * 4H):
+ *   w_ih  bf16 [dirs * 4H, in] (in = embed_dim for layer 0, else dirs * H), bias fp32 [dirs * 4H] = b_ih + b_hh,
+ *   w_hh  bf16 [dirs * 4H, H].
+ * sb_laser2_forward is sb_laser2_embed, then per layer sb_gemm_bf16 (bias epilogue) on these and sb_lstm_recurrent. */
+int sb_laser2_layer_weights(const SbLaser2* enc, int32_t layer, const void** w_ih, const float** bias, const void** w_hh);
+
+/* The embedding gather of sb_laser2_forward alone.
+ *   ids        DEVICE int64 [B, ids_row_stride >= S]; cu_seqlens DEVICE int32 [B + 1] with lengths in 0..S
+ *   table      DEVICE bf16 [vocab, D], D a positive multiple of 8, 16-byte aligned
+ *   x          DEVICE bf16 [cu[B], D], 16-byte aligned: row cu[b] + t = table[ids[b, t]] for t < len_b
+ *   pad_mask   DEVICE uint8 [cu[B]]: 1 where ids[b, t] == pad_idx, t < len_b
+ *   tail_keep  DEVICE uint8 [B]: 1 if some ids[b, t] != pad_idx with len_b <= t < S (positions >= S are not read)
+ *   err_flag   DEVICE int32: set to 1 (never cleared) when an id lies outside [0, vocab); that row of x is zero. */
+int sb_laser2_embed(const int64_t* ids, int64_t ids_row_stride, const int32_t* cu_seqlens, int32_t B, int32_t S,
+                    const void* table, int64_t vocab, int32_t D, int64_t pad_idx, void* x, uint8_t* pad_mask,
+                    uint8_t* tail_keep, int32_t* err_flag, void* stream);
 
 /* The LSTM recurrence alone (H = 512), for one layer and `num_dirs` directions.  Gate order: row / column
  * d * 4H + 128 c + 32 gate + u of the operands below is gate `gate` (i, f, g, o) of hidden unit 32 c + u of direction d.
- *   G          DEVICE bf16 [T, ldg >= num_dirs * 4H] input pre-activations X . W_ih^T + b_ih + b_hh of the packed tokens
- *   w_hh       DEVICE bf16 [num_dirs * 4H, H] in the gate order above
+ *   G          DEVICE bf16 [T, ldg] input pre-activations X . W_ih^T + b_ih + b_hh of the packed tokens; 4-byte aligned,
+ *              ldg even and >= num_dirs * 4H (only the first num_dirs * 4H columns are read)
+ *   w_hh       DEVICE bf16 [num_dirs * 4H, H] in the gate order above, 16-byte aligned
  *   cu_seqlens DEVICE int32 [B + 1]: the tokens of sequence b are rows cu[b] .. cu[b + 1] - 1
- *   tile_seqs  DEVICE int32 [num_tiles * 64]: the sequences of each 64-row tile, -1 = empty row
+ *   tile_seqs  DEVICE int32 [num_tiles * 64]: the sequences of each 64-row tile, -1 = empty row; a tile may be all -1
  * and exactly one of
- *   y          DEVICE bf16 [T, ldy]: h_t of direction d at columns d * H (the reverse direction runs from the last token)
+ *   y          DEVICE bf16 [T, ldy]: h_t of direction d at columns d * H (the reverse direction runs from the last token);
+ *              4-byte aligned, ldy even and >= num_dirs * H; only the tokens of sequences in tile_seqs and only the first
+ *              num_dirs * H columns are written
  *   pool_out   DEVICE fp32 [B, ldp]: max over the sequence's tokens of h_t, skipping tokens with pad_mask[token] != 0
  *              (DEVICE uint8 [T] or NULL), then max with padding_value where tail_keep[b] != 0 (DEVICE uint8 [B] or NULL);
- *              only sequences named in tile_seqs are written. */
+ *              -inf when nothing is left; 8-byte aligned, ldp even and >= num_dirs * H; only the rows of sequences named in
+ *              tile_seqs and only the first num_dirs * H columns are written.
+ * A leading dimension or an alignment outside these rules is SB_ERR_INVALID, refused before any launch. */
 int sb_lstm_recurrent(const void* G, int64_t ldg, const void* w_hh, const int32_t* cu_seqlens, const int32_t* tile_seqs,
                       int32_t num_tiles, int32_t num_dirs, void* y, int64_t ldy, float* pool_out, int64_t ldp,
                       const uint8_t* pad_mask, const uint8_t* tail_keep, float padding_value, void* stream);

@@ -195,6 +195,10 @@ _SIGNATURES = {
     "sb_laser2_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                     C.c_void_p, C.c_size_t, C.c_void_p]),
     "sb_laser2_check_inputs": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "sb_laser2_layer_weights": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                          C.POINTER(C.c_void_p)]),
+    "sb_laser2_embed": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int32,
+                                  C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_lstm_recurrent": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                     C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float,
                                     C.c_void_p]),

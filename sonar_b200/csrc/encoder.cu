@@ -205,7 +205,7 @@ static Workspace carve(const SbEncoder* e, int32_t max_batch, int64_t max_tokens
 extern "C" {
 
 const char* sb_last_error(void) { return g_err; }
-int sb_version(void) { return 111; }
+int sb_version(void) { return 112; }
 
 int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbEncoder** out) {
   if (!cfg || !w || !out) { set_last_error("sb_encoder_create: null argument"); return SB_ERR_INVALID; }

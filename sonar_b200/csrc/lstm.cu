@@ -355,6 +355,8 @@ struct LaserWs {
 
 int lstm_tiles(long long B) { return (int)((B + kLstmRows - 1) / kLstmRows); }
 
+bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 }  // namespace
 }  // namespace sb
 
@@ -406,6 +408,10 @@ int sb_laser2_create(const SbLaser2Config* cfg, const SbLaser2Weights* w, SbLase
   }
   const int dirs = cfg->bidirectional ? 2 : 1, L = cfg->num_layers;
   if (!w->embed || !w->layers) { set_last_error("sb_laser2_create: missing weight pointer"); return SB_ERR_INVALID; }
+  if (!aligned_to(w->embed, 16)) {  // the gather reads the table as int4
+    set_last_error("sb_laser2_create: the embedding table must be 16-byte aligned");
+    return SB_ERR_INVALID;
+  }
   for (int i = 0; i < L * dirs; ++i)
     if (has_null_pointer(w->layers[i])) {
       set_last_error("sb_laser2_create: layer %d direction %d has a null weight pointer", i / dirs, i % dirs);
@@ -525,11 +531,60 @@ int sb_laser2_check_inputs(SbLaser2* e, void* stream_v) {
   return e->err_flag.check("sb_laser2_forward", reinterpret_cast<cudaStream_t>(stream_v));
 }
 
+int sb_laser2_layer_weights(const SbLaser2* e, int32_t layer, const void** w_ih, const float** bias, const void** w_hh) {
+  if (!e || !w_ih || !bias || !w_hh || layer < 0 || layer >= e->cfg.num_layers) {
+    set_last_error("sb_laser2_layer_weights: null argument or layer %d outside [0, %d)", layer, e ? e->cfg.num_layers : 0);
+    return SB_ERR_INVALID;
+  }
+  *w_ih = e->w_ih[layer];
+  *bias = e->bias[layer];
+  *w_hh = e->w_hh[layer];
+  return SB_OK;
+}
+
+int sb_laser2_embed(const int64_t* ids, int64_t ids_row_stride, const int32_t* cu_seqlens, int32_t B, int32_t S,
+                    const void* table, int64_t vocab, int32_t D, int64_t pad_idx, void* x, uint8_t* pad_mask,
+                    uint8_t* tail_keep, int32_t* err_flag, void* stream) {
+  if (!ids || !cu_seqlens || !table || !x || !pad_mask || !tail_keep || !err_flag) {
+    set_last_error("sb_laser2_embed: null pointer");
+    return SB_ERR_INVALID;
+  }
+  if (B <= 0 || S <= 0 || ids_row_stride < S || vocab <= 0 || D <= 0 || D % 8 != 0) {
+    set_last_error("sb_laser2_embed: bad shape (B=%d, S=%d, ids_row_stride=%lld, vocab=%lld, D=%d; D a positive multiple of 8)",
+                   B, S, (long long)ids_row_stride, (long long)vocab, D);
+    return SB_ERR_INVALID;
+  }
+  if (!aligned_to(table, 16) || !aligned_to(x, 16)) {  // rows move as int4
+    set_last_error("sb_laser2_embed: table and x must be 16-byte aligned");
+    return SB_ERR_INVALID;
+  }
+  int sms = 0;
+  if (int rc = require_hopper("sb_laser2_embed", &sms)) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  laser_embed_kernel<<<B, 128, 0, s>>>(ids, ids_row_stride, cu_seqlens, S, reinterpret_cast<const int4*>(table), vocab, D,
+                                       pad_idx, reinterpret_cast<int4*>(x), pad_mask, tail_keep, err_flag);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return SB_OK;
+}
+
 int sb_lstm_recurrent(const void* G, int64_t ldg, const void* w_hh, const int32_t* cu_seqlens, const int32_t* tile_seqs,
                       int32_t num_tiles, int32_t num_dirs, void* y, int64_t ldy, float* pool_out, int64_t ldp,
                       const uint8_t* pad_mask, const uint8_t* tail_keep, float padding_value, void* stream) {
   if (!G || !w_hh || !cu_seqlens || !tile_seqs || (!y) == (!pool_out)) {
     set_last_error("sb_lstm_recurrent: null pointer, or not exactly one of y / pool_out");
+    return SB_ERR_INVALID;
+  }
+  if (num_dirs < 1 || num_dirs > 2) { set_last_error("sb_lstm_recurrent: num_dirs %d (1 or 2)", num_dirs); return SB_ERR_INVALID; }
+  // the kernel loads G in bf16 pairs, stores y in bf16 pairs and the pool in fp32 pairs, and copies W_hh in 16-byte pieces
+  const long long width = (long long)num_dirs * kLstmH;
+  const long long ld_out = y ? ldy : ldp;
+  if (ldg < 4 * width || ldg % 2 != 0 || ld_out < width || ld_out % 2 != 0) {
+    set_last_error("sb_lstm_recurrent: leading dimensions must be even with ldg >= %lld and %s >= %lld (got ldg=%lld, %s=%lld)",
+                   4 * width, y ? "ldy" : "ldp", width, (long long)ldg, y ? "ldy" : "ldp", ld_out);
+    return SB_ERR_INVALID;
+  }
+  if (!aligned_to(G, 4) || !aligned_to(w_hh, 16) || (y && !aligned_to(y, 4)) || (pool_out && !aligned_to(pool_out, 8))) {
+    set_last_error("sb_lstm_recurrent: G and y must be 4-byte aligned, pool_out 8-byte aligned and w_hh 16-byte aligned");
     return SB_ERR_INVALID;
   }
   int sms = 0;

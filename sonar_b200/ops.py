@@ -411,14 +411,16 @@ def lstm_gate_rows(hidden_size: int = 512, num_dirs: int = 1) -> Tensor:
 
 def lstm_recurrent(g: Tensor, w_hh: Tensor, cu_seqlens: Tensor, tile_seqs: Tensor, num_dirs: int, *,
                    pool: bool = False, pad_mask: Optional[Tensor] = None, tail_keep: Optional[Tensor] = None,
-                   padding_value: float = 0.0) -> Tensor:
+                   padding_value: float = 0.0, out: Optional[Tensor] = None) -> Tensor:
     """The LSTM recurrence (H = 512) of one layer on packed tokens, everything in ``lstm_gate_rows`` order:
-    g bf16 [T, num_dirs * 4H] input pre-activations (x . W_ih^T + b_ih + b_hh), w_hh bf16 [num_dirs * 4H, H],
-    cu_seqlens int32 [B + 1], tile_seqs int32 [tiles * 64] (sequence per tile row, -1 = empty).  Returns the outputs
-    bf16 [T, num_dirs * H], or with ``pool`` fp32 [B, num_dirs * H]: the max over each sequence's tokens, skipping those
-    with pad_mask (uint8 [T]) set, then max with ``padding_value`` where tail_keep (uint8 [B]) is set; rows of sequences
-    missing from tile_seqs are left uninitialised."""
-    _need_cuda(g, w_hh, cu_seqlens, tile_seqs, pad_mask, tail_keep)
+    g bf16 [T, num_dirs * 4H] input pre-activations (x . W_ih^T + b_ih + b_hh; may be a column view of a wider buffer),
+    w_hh bf16 [num_dirs * 4H, H], cu_seqlens int32 [B + 1], tile_seqs int32 [tiles * 64] (sequence per tile row,
+    -1 = empty).  Returns the outputs bf16 [T, num_dirs * H], or with ``pool`` fp32 [B, num_dirs * H]: the max over each
+    sequence's tokens, skipping those with pad_mask (uint8 [T]) set, then max with ``padding_value`` where tail_keep
+    (uint8 [B]) is set; rows of sequences missing from tile_seqs are left uninitialised.  ``out`` may give that output
+    as a caller-owned view with unit column stride (its row stride may be wider than the data); only its rows and
+    columns are written."""
+    _need_cuda(g, w_hh, cu_seqlens, tile_seqs, pad_mask, tail_keep, out)
     assert g.dtype == torch.bfloat16 and w_hh.dtype == torch.bfloat16 and g.stride(1) == 1 and w_hh.is_contiguous()
     assert cu_seqlens.dtype == torch.int32 and tile_seqs.dtype == torch.int32 and tile_seqs.numel() % LSTM_TILE_ROWS == 0
     h = w_hh.shape[1]
@@ -426,17 +428,73 @@ def lstm_recurrent(g: Tensor, w_hh: Tensor, cu_seqlens: Tensor, tile_seqs: Tenso
     for m in (pad_mask, tail_keep):
         assert m is None or m.dtype == torch.uint8
     t, b = g.shape[0], cu_seqlens.numel() - 1
-    if pool:
-        out = torch.empty((b, num_dirs * h), dtype=torch.float32, device=g.device)
-        y, pool_out, ld = None, out, out.stride(0)
-    else:
-        out = torch.empty((t, num_dirs * h), dtype=torch.bfloat16, device=g.device)
-        y, pool_out, ld = out, None, out.stride(0)
+    shape, dtype = ((b, num_dirs * h), torch.float32) if pool else ((t, num_dirs * h), torch.bfloat16)
+    if out is None:
+        out = torch.empty(shape, dtype=dtype, device=g.device)
+    assert out.dtype == dtype and tuple(out.shape) == shape and out.stride(1) == 1
+    y, pool_out, ld = (None, out, out.stride(0)) if pool else (out, None, out.stride(0))
     rc = _lib.load().sb_lstm_recurrent(g.data_ptr(), g.stride(0), w_hh.data_ptr(), cu_seqlens.data_ptr(), tile_seqs.data_ptr(),
                                        tile_seqs.numel() // LSTM_TILE_ROWS, num_dirs, _ptr(y), ld, _ptr(pool_out), ld,
                                        _ptr(pad_mask), _ptr(tail_keep), padding_value, _stream())
     _lib.check(rc, "sb_lstm_recurrent")
     return out
+
+
+def laser_embed(ids: Tensor, cu_seqlens: Tensor, table: Tensor, pad_idx: int, *, seq_len: Optional[int] = None,
+                out: Optional[tuple] = None, flag: Optional[Tensor] = None):
+    """The LASER2 embedding gather (``sb_laser2_embed``): ids int64 [B, W] with unit column stride (seq_len <= W,
+    default W), cu_seqlens int32 [B + 1] (lengths <= seq_len), table bf16 [V, D] -> (x bf16 [T, D], pad uint8 [T],
+    tail uint8 [B], flag int32 [1]): x row cu[b] + t = table[ids[b, t]], pad = (id == pad_idx), tail[b] = some id at
+    len_b <= t < seq_len differs from pad_idx; an id outside [0, V) gathers zeros and sets flag[0] to 1 (``flag`` is
+    not cleared first).  ``out`` optionally gives (x, pad, tail), pad and tail contiguous with at least T and B
+    entries."""
+    _need_cuda(ids, cu_seqlens, table, flag)
+    assert ids.dtype == torch.int64 and ids.dim() == 2 and ids.stride(1) == 1 and cu_seqlens.dtype == torch.int32
+    assert table.dtype == torch.bfloat16 and table.is_contiguous()
+    b = ids.shape[0]
+    s = ids.shape[1] if seq_len is None else seq_len
+    (v, d), t = table.shape, int(cu_seqlens[-1])
+    assert cu_seqlens.numel() == b + 1 and s <= ids.shape[1] <= ids.stride(0)
+    if out is None:
+        out = (torch.empty((t, d), dtype=torch.bfloat16, device=ids.device), torch.empty(t, dtype=torch.uint8, device=ids.device),
+               torch.empty(b, dtype=torch.uint8, device=ids.device))
+    x, pad, tail = out
+    _need_cuda(x, pad, tail)
+    assert x.dtype == torch.bfloat16 and x.shape == (t, d) and x.is_contiguous()
+    assert pad.dtype == tail.dtype == torch.uint8 and pad.is_contiguous() and tail.is_contiguous()
+    assert pad.numel() >= t and tail.numel() >= b
+    if flag is None:
+        flag = torch.zeros(1, dtype=torch.int32, device=ids.device)
+    assert flag.dtype == torch.int32
+    rc = _lib.load().sb_laser2_embed(ids.data_ptr(), ids.stride(0), cu_seqlens.data_ptr(), b, s, table.data_ptr(), v, d,
+                                     pad_idx, x.data_ptr(), pad.data_ptr(), tail.data_ptr(), flag.data_ptr(), _stream())
+    _lib.check(rc, "sb_laser2_embed")
+    return x, pad, tail, flag
+
+
+class _DeviceArray:
+    """A borrowed device buffer seen through ``__cuda_array_interface__`` (no copy)."""
+
+    def __init__(self, ptr: int, shape: tuple, typestr: str) -> None:
+        self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (ptr, False), "version": 3}
+
+
+def laser2_layer_weights(model, layer: int):
+    """Copies of a ``B200LaserLstmEncoder``'s repacked weights of one layer (``sb_laser2_layer_weights``):
+    (w_ih bf16 [dirs * 4H, in], bias fp32 [dirs * 4H], w_hh bf16 [dirs * 4H, H]), rows in ``lstm_gate_rows`` order."""
+    cfg = model.config
+    dirs, h = (2 if cfg.bidirectional else 1), cfg.hidden_size
+    n, k = dirs * 4 * h, (cfg.model_dim if layer == 0 else dirs * h)
+    w_ih, bias, w_hh = C.c_void_p(), C.c_void_p(), C.c_void_p()
+    _lib.check(model._lib.sb_laser2_layer_weights(model._handle, layer, C.byref(w_ih), C.byref(bias), C.byref(w_hh)),
+               "sb_laser2_layer_weights")
+    dev = model.device
+
+    def view(p, shape, typestr):
+        return torch.as_tensor(_DeviceArray(p.value, shape, typestr), device=dev).clone()
+
+    return (view(w_ih, (n, k), "<i2").view(torch.bfloat16), view(bias, (n,), "<f4"),
+            view(w_hh, (n, h), "<i2").view(torch.bfloat16))
 
 
 def blaser_featurize(src: Tensor, mt: Tensor, ref: Optional[Tensor], input_form: str, *, normalize: bool = False,
