@@ -159,9 +159,9 @@ int sb_encoder_forward_host(SbEncoder* enc, const int64_t* ids_host, const int32
  * duration can be read INSIDE a real step.  Pass NULL, NULL to switch it off. */
 int sb_encoder_profile_ffn1(SbEncoder* enc, void* start_event, void* stop_event);
 
-/* Checks the sticky device-side input flag (token id out of range) of the last forwards;
+/* Reads and clears the handle's sticky device-side input flag (token id out of range in a forward since the last check);
  * synchronises `stream`.  Returns SB_OK or SB_ERR_INPUT. */
-int sb_encoder_check_inputs(SbEncoder* enc, void* workspace, void* stream);
+int sb_encoder_check_inputs(SbEncoder* enc, void* stream);
 
 /* ---- individual kernels (used by the parity tests and the micro-benchmarks) ---- */
 
@@ -304,6 +304,7 @@ typedef struct SbDecoderWeights {
   const SbDecoderLayerWeights* layers; /* HOST array */
 } SbDecoderWeights;
 
+/* Allocates the handle's 256-byte input-check flag; sb_decoder_begin and sb_decoder_step never allocate. */
 int sb_decoder_create(const SbDecoderConfig* cfg, const SbDecoderWeights* w, SbDecoder** out);
 void sb_decoder_destroy(SbDecoder* dec);
 /* workspace for num_sentences x beam hypotheses of at most max_len positions (holds the KV caches) */
@@ -323,7 +324,9 @@ int sb_decoder_step(SbDecoder* dec, const int64_t* tokens, const int32_t* table,
                     int32_t beam, int32_t max_len, float* out_lprob, int32_t* out_tok, float* out_eos_lprob,
                     const int64_t* probe_tokens, float* out_probe_lprob, void* workspace, size_t workspace_bytes,
                     void* stream);
-int sb_decoder_check_inputs(SbDecoder* dec, void* workspace, void* stream);
+/* Reads and clears the handle's sticky device-side input flag (token id outside [0, vocab_size) in a step since the last
+ * check; sb_decoder_begin leaves it as it is); synchronises `stream`.  Returns SB_OK or SB_ERR_INPUT. */
+int sb_decoder_check_inputs(SbDecoder* dec, void* stream);
 
 /* The decoder step's kernels, launched as sb_decoder_step launches them (R hypothesis rows, DEVICE pointers).
  *
@@ -431,21 +434,22 @@ typedef struct SbSpeechWeights {
   const SbPoolerLayerWeights* pooler;
 } SbSpeechWeights;
 
-/* Allocates the handle's own device memory, the absorbed cross-attention weights of every pooler layer (as for
+/* Allocates the handle's own memory: on the device the absorbed cross-attention weights of every pooler layer (as for
  * sb_encoder_create with E = D and Hd = num_heads: 2 * Hd * D * D * 2 + (Hd * D + D) * 4 bytes = 64 MB per layer at
- * D = 1024, so 192 MB for `english` and 384 MB for `non_english`), and synchronises the device once.
- * sb_speech_encoder_forward never allocates. */
+ * D = 1024, so 192 MB for `english` and 384 MB for `non_english`), on the host a pinned ring of 8 x 65 536 int32 through
+ * which the forwards stage their lengths.  Synchronises the device once.  sb_speech_encoder_forward never allocates. */
 int sb_speech_encoder_create(const SbSpeechConfig* cfg, const SbSpeechWeights* w, SbSpeechEncoder** out);
 void sb_speech_encoder_destroy(SbSpeechEncoder* enc);
 int sb_speech_encoder_workspace_bytes(const SbSpeechEncoder* enc, int32_t batch, int64_t total_positions,
                                       int32_t max_positions, size_t* bytes);
-/* fbank DEVICE fp32 [batch, padded_frames, 80] (sb_fbank output); cu_dev DEVICE int32 [batch+1] cumulative positions,
- * lens_host HOST int32 [batch] positions per utterance (= frames // 2); relpos_table DEVICE bf16 [relpos_rows, D] with
+/* fbank DEVICE fp32 [batch, padded_frames, 80] (sb_fbank output); lens_host HOST int32 [batch] positions per utterance
+ * (= frames // 2) in 1..padded_frames / 2; relpos_table DEVICE bf16 [relpos_rows, D] with
  * relpos_rows = roundup(2*max_len - 1, 256), row k = sinusoid of relative position (max_len - 1 - k), zero rows after
- * 2*max_len - 1; out DEVICE fp32 [batch, D]; encoded_packed DEVICE fp32 [total_positions, D] or NULL. */
-int sb_speech_encoder_forward(SbSpeechEncoder* enc, const float* fbank, int32_t padded_frames, const int32_t* cu_dev,
-                              const int32_t* lens_host, int32_t batch, const void* relpos_table, int32_t relpos_rows,
-                              float* out, float* encoded_packed, void* workspace, size_t workspace_bytes, void* stream);
+ * 2*max_len - 1; out DEVICE fp32 [batch, D]; encoded_packed DEVICE fp32 [total_positions, D] or NULL.
+ * batch <= 65535.  Asynchronous on `stream` (does not synchronise). */
+int sb_speech_encoder_forward(SbSpeechEncoder* enc, const float* fbank, int32_t padded_frames, const int32_t* lens_host,
+                              int32_t batch, const void* relpos_table, int32_t relpos_rows, float* out,
+                              float* encoded_packed, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- xsim cosine k-NN / margin mining over sentence embeddings (BASELINE.json config 5) ----
  * Not a reference interface: the reference only ever does normalize + matmul

@@ -123,7 +123,7 @@ _SIGNATURES = {
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                           C.c_void_p]),
     "sb_encoder_profile_ffn1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
-    "sb_encoder_check_inputs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_encoder_check_inputs": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_gemm_bf16": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
@@ -152,7 +152,7 @@ _SIGNATURES = {
     "sb_decoder_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                   C.c_void_p]),
-    "sb_decoder_check_inputs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_decoder_check_inputs": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_decoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_int32,
                                    C.c_void_p, C.c_void_p]),
     "sb_decoder_attention": (C.c_int, [C.c_void_p] * 4 + [C.c_int32] * 4 + [C.c_void_p] * 2),
@@ -168,9 +168,8 @@ _SIGNATURES = {
     "sb_speech_encoder_create": (C.c_int, [C.POINTER(SbSpeechConfig), C.POINTER(SbSpeechWeights), C.POINTER(C.c_void_p)]),
     "sb_speech_encoder_destroy": (None, [C.c_void_p]),
     "sb_speech_encoder_workspace_bytes": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.POINTER(C.c_size_t)]),
-    "sb_speech_encoder_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
-                                            C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
-                                            C.c_void_p]),
+    "sb_speech_encoder_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                            C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "sb_xsim_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]),
     "sb_xsim_knn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                               C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -9,6 +9,7 @@
 #include "sonar_b200_internal.h"
 
 #include <algorithm>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -236,7 +237,7 @@ int sb_blaser_create(const SbBlaserConfig* cfg, const SbBlaserWeights* w, SbBlas
   if (!aligned16(w->w[L])) { set_last_error("sb_blaser_create: the output weight must be 16-byte aligned"); return SB_ERR_INVALID; }
   int num_sms = 0;
   if (int rc = require_hopper("sb_blaser_create", &num_sms)) return rc;
-  SbBlaser* e = new (std::nothrow) SbBlaser();
+  std::unique_ptr<SbBlaser> e(new (std::nothrow) SbBlaser());
   if (!e) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   e->input_form = cfg->input_form;
   e->E = cfg->embedding_dim;
@@ -251,7 +252,7 @@ int sb_blaser_create(const SbBlaserConfig* cfg, const SbBlaserWeights* w, SbBlas
   e->b_out = w->b[L];
   e->cta_group = cfg->cta_group == 1 ? 1 : 2;
   e->num_sms = cfg->num_sms > 0 ? cfg->num_sms : num_sms;
-  *out = e;
+  *out = e.release();
   return SB_OK;
 }
 

@@ -20,6 +20,8 @@
 #include "sonar_b200_internal.h"
 
 #include <math_constants.h>
+#include <algorithm>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -539,11 +541,14 @@ struct SbSpeechEncoder {
   std::vector<SbConformerLayerWeights> layers;
   AttentionPooler pooler;
   int num_sms;
+  static constexpr int kMaxBatch = 65535;  // grid z of the attention and conv kernels
+  StagingRing staging;  // cu_seqlens
 };
 
 namespace {
 
 struct SpWs {
+  int32_t* cu;          // [B+1]
   __nv_bfloat16* a192;  // [T,192]
   float* x;             // [T,D]
   __nv_bfloat16* h;     // [T,D]
@@ -563,6 +568,7 @@ SpWs carve_sp(const SbSpeechEncoder* e, int B, long long T, int smax, void* base
   Carver c(base);
   SpWs w;
   const size_t t = (size_t)T;
+  w.cu = c.take<int32_t>(sizeof(int32_t) * ((size_t)B + 1));
   w.a192 = c.take<__nv_bfloat16>(t * kFeatPad * 2);
   w.x = c.take<float>(t * D * 4);
   w.h = c.take<__nv_bfloat16>(t * D * 2);
@@ -602,19 +608,18 @@ int sb_speech_encoder_create(const SbSpeechConfig* cfg, const SbSpeechWeights* w
     }
   int num_sms = 0;
   if (int rc = require_hopper("sb_speech_encoder_create", &num_sms)) return rc;
-  SbSpeechEncoder* e = new (std::nothrow) SbSpeechEncoder();
+  std::unique_ptr<SbSpeechEncoder> e(new (std::nothrow) SbSpeechEncoder());
   if (!e) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   e->cfg = *cfg;
   e->w = *w;
   e->layers.assign(w->layers, w->layers + cfg->num_layers);
   e->num_sms = num_sms;
+  if (int rc = e->staging.create("sb_speech_encoder_create", SbSpeechEncoder::kMaxBatch + 1)) return rc;
   // the projection has no bias: zeros; every GEMM of this engine may take the weight-streaming path
   if (int rc = e->pooler.create("sb_speech_encoder_create", w->pooler, cfg->pooler_layers, w->pooler_q0, w->proj_w, w->zeros,
-                                D, D, cfg->pooler_ffn_inner_dim, cfg->ln_eps, num_sms, 2, 1)) {
-    sb_speech_encoder_destroy(e);
+                                D, D, cfg->pooler_ffn_inner_dim, cfg->ln_eps, num_sms, 2, 1))
     return rc;
-  }
-  *out = e;
+  *out = e.release();
   return SB_OK;
 }
 
@@ -630,23 +635,23 @@ int sb_speech_encoder_workspace_bytes(const SbSpeechEncoder* e, int32_t B, int64
   return SB_OK;
 }
 
-int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t padded_frames, const int32_t* cu_dev,
-                              const int32_t* lens_host, int32_t B, const void* relpos_table, int32_t relpos_rows,
-                              float* out, float* encoded_packed, void* workspace, size_t workspace_bytes,
-                              void* stream_v) {
-  if (!e || !fbank || !cu_dev || !lens_host || !relpos_table || !out || !workspace) {
+int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t padded_frames, const int32_t* lens_host,
+                              int32_t B, const void* relpos_table, int32_t relpos_rows, float* out, float* encoded_packed,
+                              void* workspace, size_t workspace_bytes, void* stream_v) {
+  if (!e || !fbank || !lens_host || !relpos_table || !out || !workspace) {
     set_last_error("sb_speech_encoder_forward: null argument");
     return SB_ERR_INVALID;
   }
-  if (B <= 0 || B > 65535) { set_last_error("sb_speech_encoder_forward: bad batch size %d", B); return SB_ERR_INVALID; }
-  long long T = 0;
+  if (B <= 0 || B > SbSpeechEncoder::kMaxBatch) { set_last_error("sb_speech_encoder_forward: bad batch size %d", B); return SB_ERR_INVALID; }
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+  // ---- cu_seqlens on the host, staged through a pinned ring ----
+  int32_t* cu_h;
+  long long T;
+  int rc = e->staging.acquire(&cu_h);
+  if (!rc) rc = host_cu_seqlens("sb_speech_encoder_forward", lens_host, B, padded_frames / 2, 1, cu_h, &T);
+  if (rc) return rc;
   int smax = 0;
-  for (int b = 0; b < B; ++b) {
-    const int n = lens_host[b];
-    if (n <= 0 || 2 * n > padded_frames) { set_last_error("sb_speech_encoder_forward: lens[%d]=%d invalid", b, n); return SB_ERR_INVALID; }
-    T += n;
-    if (n > smax) smax = n;
-  }
+  for (int b = 0; b < B; ++b) smax = std::max(smax, cu_h[b + 1] - cu_h[b]);
   const int Npad = npad_of(smax);
   if (relpos_rows != Npad) {
     set_last_error("sb_speech_encoder_forward: relative-position table must have %d rows for max length %d (got %d)", Npad,
@@ -654,10 +659,11 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
     return SB_ERR_INVALID;
   }
   SpWs w;
-  int rc = bind_workspace("sb_speech_encoder_forward", workspace, workspace_bytes, &w,
-                          [&](void* p) { return carve_sp(e, B, T, smax, p); });
+  rc = bind_workspace("sb_speech_encoder_forward", workspace, workspace_bytes, &w,
+                      [&](void* p) { return carve_sp(e, B, T, smax, p); });
   if (rc) return rc;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+  SB_CUDA_CHECK(cudaMemcpyAsync(w.cu, cu_h, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice, stream));
+  if ((rc = e->staging.record(stream))) return rc;
   const int D = e->cfg.model_dim, F = e->cfg.ffn_inner_dim, H = e->cfg.num_heads;
   const float eps = e->cfg.ln_eps;
   // the mma.sync kernel (A/B runs, second implementation in the tests) is the only one for more than 2047 utterances
@@ -670,7 +676,7 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
     return gemm_bf16(g, stream);
   };
   // ---- frontend ----
-  if ((rc = speech_frontend(fbank, padded_frames, cu_dev, B, smax, e->w.front_ln_g, e->w.front_ln_b, eps, w.a192, stream)))
+  if ((rc = speech_frontend(fbank, padded_frames, w.cu, B, smax, e->w.front_ln_g, e->w.front_ln_b, eps, w.a192, stream)))
     return rc;
   if ((rc = gemm(w.a192, kFeatPad, e->w.front_w, kFeatPad, w.x, D, 1, e->w.front_b, (int)T, D, kFeatPad, EPI_BIAS))) return rc;
   // ---- conformer blocks ----
@@ -684,14 +690,14 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
     if ((rc = layernorm_bf16(w.x, L.attn_ln_g, L.attn_ln_b, eps, w.h, T, D, stream))) return rc;
     if ((rc = gemm(w.h, D, L.wqkv, D, w.big, 3 * D, 0, L.bqkv, (int)T, 3 * D, D, EPI_BIAS))) return rc;
     if ((rc = gemm(relpos_table, D, L.wr, D, w.p, D, 0, e->w.zeros, Npad, D, D, EPI_BIAS))) return rc;
-    if ((rc = attention_relpos(w.big, w.p, L.u_bias, L.v_bias, cu_dev, B, H, T, Npad, smax, attn_impl, w.qu, w.qv, w.vp, w.h,
+    if ((rc = attention_relpos(w.big, w.p, L.u_bias, L.v_bias, w.cu, B, H, T, Npad, smax, attn_impl, w.qu, w.qv, w.vp, w.h,
                                e->num_sms, stream)))
       return rc;
     if ((rc = gemm(w.h, D, L.wo, D, w.x, D, 1, L.bo, (int)T, D, D, EPI_BIAS_RESIDUAL))) return rc;
     // (c) convolution module
     if ((rc = layernorm_bf16(w.x, L.conv_ln_g, L.conv_ln_b, eps, w.h, T, D, stream))) return rc;
     if ((rc = gemm(w.h, D, L.pw1, D, w.big, 2 * D, 0, e->w.zeros, (int)T, 2 * D, D, EPI_BIAS))) return rc;
-    if ((rc = conformer_conv(w.big, cu_dev, B, smax, D, L.dw, L.bn_scale, L.bn_shift, w.h, stream))) return rc;
+    if ((rc = conformer_conv(w.big, w.cu, B, smax, D, L.dw, L.bn_scale, L.bn_shift, w.h, stream))) return rc;
     if ((rc = gemm(w.h, D, L.pw2, D, w.x, D, 1, e->w.zeros, (int)T, D, D, EPI_BIAS_RESIDUAL))) return rc;
     // (d) half-step FFN 2
     if ((rc = layernorm_bf16(w.x, L.ffn2_ln_g, L.ffn2_ln_b, eps, w.h, T, D, stream))) return rc;
@@ -703,7 +709,7 @@ int sb_speech_encoder_forward(SbSpeechEncoder* e, const float* fbank, int32_t pa
   // ---- model.layer_norm (fp32 in place, bf16 copy = pooler memory) ----
   if ((rc = layernorm_dual(w.x, e->w.final_ln_g, e->w.final_ln_b, eps, w.x, w.h, T, D, stream))) return rc;
   if (encoded_packed) SB_CUDA_CHECK(cudaMemcpyAsync(encoded_packed, w.x, sizeof(float) * (size_t)T * D, cudaMemcpyDeviceToDevice, stream));
-  return e->pooler.forward(w.pool, w.h, cu_dev, B, out, stream);
+  return e->pooler.forward(w.pool, w.h, w.cu, B, out, stream);
 }
 
 int sb_attention_relpos(const void* qkv, const void* p, const float* u_bias, const float* v_bias, const int32_t* cu_seqlens,

@@ -24,6 +24,7 @@
 #include "sonar_b200_internal.h"
 
 #include <math_constants.h>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -362,6 +363,7 @@ struct SbDecoder {
   const float* final_ln_g;
   const float* final_ln_b;
   std::vector<SbDecoderLayerWeights> layers;
+  InputFlag err_flag;  // token id out of range, cleared by sb_decoder_check_inputs
   int num_sms;
 };
 
@@ -370,7 +372,6 @@ namespace {
 constexpr long long kSplitkFlags = 4096;  // >= 4 * (tile pairs of an [R, D] residual GEMM) whenever splitting can pay
 
 struct DecWs {
-  int32_t* err_flag;      // first buffer: sb_decoder_check_inputs finds it at the workspace base
   int* splitk_flags;      // [kSplitkFlags] hand-over counters of the split-K residual GEMMs (zeroed by sb_decoder_begin)
   float* x;               // [R, D] fp32 residual stream of the current step
   __nv_bfloat16* h;       // [R, D]
@@ -394,7 +395,6 @@ DecWs carve_dec(const SbDecoder* d, int N, int beam, int Tmax, void* base) {
   Carver c(base);
   DecWs w;
   w.n_chunks = gemm_topk_chunks((int)R, (int)d->cfg.vocab_size, 2, d->num_sms);
-  w.err_flag = c.take<int32_t>(256);
   w.splitk_flags = c.take<int>(kSplitkFlags * sizeof(int));
   w.x = c.take<float>(R * D * 4);
   w.h = c.take<__nv_bfloat16>(R * D * 2);
@@ -459,7 +459,7 @@ int sb_decoder_create(const SbDecoderConfig* cfg, const SbDecoderWeights* w, SbD
     }
   int num_sms = 0;
   if (int rc = require_hopper("sb_decoder_create", &num_sms)) return rc;
-  SbDecoder* d = new (std::nothrow) SbDecoder();
+  std::unique_ptr<SbDecoder> d(new (std::nothrow) SbDecoder());
   if (!d) { set_last_error("out of host memory"); return SB_ERR_INVALID; }
   d->cfg = *cfg;
   d->embed = w->embed;
@@ -468,7 +468,8 @@ int sb_decoder_create(const SbDecoderConfig* cfg, const SbDecoderWeights* w, SbD
   d->final_ln_b = w->final_ln_b;
   d->layers.assign(w->layers, w->layers + cfg->num_layers);
   d->num_sms = num_sms;
-  *out = d;
+  if (int rc = d->err_flag.create("sb_decoder_create")) return rc;
+  *out = d.release();
   return SB_OK;
 }
 
@@ -491,7 +492,6 @@ int sb_decoder_begin(SbDecoder* d, const float* embeddings, int32_t N, int32_t b
   if (!embeddings) { set_last_error("sb_decoder_begin: null embeddings"); return SB_ERR_INVALID; }
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   const int D = d->cfg.model_dim;
-  SB_CUDA_CHECK(cudaMemsetAsync(w.err_flag, 0, sizeof(int32_t), stream));
   SB_CUDA_CHECK(cudaMemsetAsync(w.splitk_flags, 0, kSplitkFlags * sizeof(int), stream));
   const long long n = (long long)N * D;
   cast_bf16_kernel<<<(unsigned)((n / 4 + 255) / 256 + 1), 256, 0, stream>>>(embeddings, w.ebf, n);
@@ -528,7 +528,7 @@ int sb_decoder_step(SbDecoder* d, const int64_t* tokens, const int32_t* table, i
   if ((rc = check_decoder_attention("sb_decoder_step", t, max_len, R, H))) return rc;
   const __nv_bfloat16* embed = reinterpret_cast<const __nv_bfloat16*>(d->embed);
   if ((rc = decoder_embed(tokens, embed, d->cfg.vocab_size, d->pos_table + (size_t)t * D, D, d->cfg.embed_scale, w.x, R,
-                          w.err_flag, stream)))
+                          d->err_flag.dev, stream)))
     return rc;
   // Every GEMM of a step may take the weight-streaming path; the residual ones may split K when their tiles leave SM
   // pairs idle (2 560 rows).
@@ -558,17 +558,9 @@ int sb_decoder_step(SbDecoder* d, const int64_t* tokens, const int32_t* table, i
                             w.cand_idx, w.lse_part, out_lprob, out_tok, out_eos_lprob, out_probe_lprob, d->num_sms, stream);
 }
 
-int sb_decoder_check_inputs(SbDecoder* d, void* workspace, void* stream_v) {
-  if (!d || !workspace) { set_last_error("sb_decoder_check_inputs: null argument"); return SB_ERR_INVALID; }
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  int32_t flag = 0;
-  SB_CUDA_CHECK(cudaMemcpyAsync(&flag, workspace_base(workspace), sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
-  SB_CUDA_CHECK(cudaStreamSynchronize(stream));
-  if (flag != 0) {
-    set_last_error("token id outside [0, vocab_size) fed to the decoder");
-    return SB_ERR_INPUT;
-  }
-  return SB_OK;
+int sb_decoder_check_inputs(SbDecoder* d, void* stream_v) {
+  if (!d) { set_last_error("sb_decoder_check_inputs: null argument"); return SB_ERR_INVALID; }
+  return d->err_flag.check("sb_decoder_step", reinterpret_cast<cudaStream_t>(stream_v));
 }
 
 int sb_decoder_embed(const int64_t* tokens, const void* embed, int64_t vocab, const float* pos_row, int32_t D, float scale,

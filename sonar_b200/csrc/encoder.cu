@@ -205,7 +205,7 @@ static Workspace carve(const SbEncoder* e, int32_t max_batch, int64_t max_tokens
 extern "C" {
 
 const char* sb_last_error(void) { return g_err; }
-int sb_version(void) { return 112; }
+int sb_version(void) { return 113; }
 
 int sb_encoder_create(const SbEncoderConfig* cfg, const SbEncoderWeights* w, SbEncoder** out) {
   if (!cfg || !w || !out) { set_last_error("sb_encoder_create: null argument"); return SB_ERR_INVALID; }
@@ -440,8 +440,7 @@ int sb_encoder_profile_ffn1(SbEncoder* e, void* start_event, void* stop_event) {
   return SB_OK;
 }
 
-int sb_encoder_check_inputs(SbEncoder* e, void* workspace, void* stream_v) {
-  (void)workspace;  // (kept in the signature; the flag lives in the handle since v101)
+int sb_encoder_check_inputs(SbEncoder* e, void* stream_v) {
   if (!e) { set_last_error("sb_encoder_check_inputs: null argument"); return SB_ERR_INVALID; }
   return e->err_flag.check("sb_encoder_forward", reinterpret_cast<cudaStream_t>(stream_v));
 }

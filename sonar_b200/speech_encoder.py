@@ -157,16 +157,13 @@ class B200SpeechEncoderModel(EngineModel):
         if smax not in self._relpos:
             self._relpos = {smax: relative_position_table(smax, self.model_dim, rows).to(self.device, torch.bfloat16)}
         rel = self._relpos[smax]
-        cu = torch.zeros(n + 1, dtype=torch.int32)
-        cu[1:] = torch.cumsum(torch.tensor(lens), 0).to(torch.int32)
-        cu_d = cu.to(self.device)
         ws = self._ensure_workspace(n, total, smax)
         out = torch.empty((n, self.model_dim), dtype=torch.float32, device=self.device)
         enc = torch.empty((total, self.model_dim), dtype=torch.float32, device=self.device) if self.return_encoded_seqs else None
         lens_c = (C.c_int32 * n)(*lens)
         with torch.cuda.device(self.device):
             rc = self._lib.sb_speech_encoder_forward(
-                self._handle, fb.data_ptr(), t, cu_d.data_ptr(), lens_c, n, rel.data_ptr(), rows, out.data_ptr(),
+                self._handle, fb.data_ptr(), t, lens_c, n, rel.data_ptr(), rows, out.data_ptr(),
                 enc.data_ptr() if enc is not None else None, ws.data_ptr(), ws.numel(), self._stream())
         _lib.check(rc, "sb_speech_encoder_forward")
         return SonarEncoderOutput(encoded_seqs=enc, sentence_embeddings=out, padding_mask=batch.padding_mask)

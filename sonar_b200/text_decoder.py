@@ -165,6 +165,5 @@ class B200TextDecoderModel(EngineModel):
         return (lp, tok, eos) if probe is None else (lp, tok, eos, probe_lp)
 
     def check_inputs(self) -> None:
-        if self._workspace is not None:
-            _lib.check(self._lib.sb_decoder_check_inputs(self._handle, self._workspace.data_ptr(), self._stream()),
-                       "sb_decoder_check_inputs")
+        """Raise ``ValueError`` if a step since the last check was fed a token id outside the vocabulary."""
+        _lib.check(self._lib.sb_decoder_check_inputs(self._handle, self._stream()), "sb_decoder_check_inputs")

@@ -262,11 +262,8 @@ class B200TextEncoderModel(EngineModel):
                    "sb_encoder_profile_ffn1")
 
     def check_inputs(self) -> None:
-        """Raise ``ValueError`` if the last batch contained a token id outside the vocabulary."""
-        if self._workspace is None:
-            return
-        _lib.check(self._lib.sb_encoder_check_inputs(self._handle, self._workspace.data_ptr(), self._stream()),
-                   "sb_encoder_check_inputs")
+        """Raise ``ValueError`` if a batch since the last check contained a token id outside the vocabulary."""
+        _lib.check(self._lib.sb_encoder_check_inputs(self._handle, self._stream()), "sb_encoder_check_inputs")
 
     # ------------------------------------------------------------------ reference static API
     @staticmethod

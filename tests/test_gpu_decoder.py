@@ -63,6 +63,32 @@ def test_teacher_forced_steps_match_oracle(small, cuda_device, n, beam, steps):
         assert bool((lp[:, -1:] >= kth - 0.25).all())
 
 
+def test_out_of_range_token_is_reported(small, cuda_device):
+    """A token id outside the vocabulary fed to one step makes check_inputs raise once: the check clears the flag.  Until
+    then the flag survives the steps and a begin that follow."""
+    _, model = small
+    n, beam, max_len = 2, 2, 8
+    r = n * beam
+    emb = _emb(n, seed=3).to(cuda_device)
+    table = torch.arange(r, dtype=torch.int32, device=cuda_device)[:, None].expand(r, max_len).contiguous()
+    good = torch.full((r,), 5, dtype=torch.int64, device=cuda_device)
+    bad = good.clone()
+    bad[1] = VOCAB
+    model.begin(emb, beam, max_len)
+    model.check_inputs()  # no earlier test fed an out-of-range token
+    model.step(bad, table, 0)
+    model.step(good, table, 1)
+    with pytest.raises(ValueError, match="vocab"):
+        model.check_inputs()
+    model.check_inputs()
+    model.step(bad, table, 2)
+    model.begin(emb, beam, max_len)
+    model.step(good, table, 0)
+    with pytest.raises(ValueError, match="vocab"):
+        model.check_inputs()
+    model.check_inputs()
+
+
 def test_beam_reordering_through_the_ancestry_table(small, cuda_device):
     """Hypothesis r continues from a DIFFERENT physical row: results must equal decoding that token history directly."""
     oracle, model = small

@@ -1,8 +1,8 @@
 """The engines' host side: every C-ABI entry point that carves the caller's workspace rejects one that is too small
 (SB_ERR_INVALID, a message that names the entry point) instead of writing past its end, the Python wrappers keep the
 weights the engines point into out of reach of ``nn.Module`` conversions, and the pinned ring through which the text
-encoder and LASER2 stage their host lengths is not rewritten while a copy still reads it.  Engines are the small
-configurations of the other GPU tests."""
+encoder, the speech encoder and LASER2 stage their host lengths is not rewritten while a copy still reads it.  Engines are
+the small configurations of the other GPU tests."""
 
 import ctypes as C
 
@@ -35,7 +35,9 @@ def engines(native_lib, cuda_device):
     return encoder, decoder, speech
 
 
-def test_too_small_workspace_is_rejected(engines, cuda_device):
+def test_too_small_workspace_is_rejected_with_host_lengths(engines, cuda_device):
+    """Every entry point that carves a workspace refuses a 1-byte one; the speech forward takes its lengths on the host
+    only, and the decoder's begin and step are refused although its layout no longer starts with an input flag."""
     from sonar_b200 import _lib
 
     encoder, decoder, speech = engines
@@ -53,7 +55,6 @@ def test_too_small_workspace_is_rejected(engines, cuda_device):
     R = n * beam
     lens = (C.c_int32 * B)(*[8] * B)      # 8 speech positions per utterance (16 fbank frames)
     rows = 256                            # relative-position table rows for 8 positions: roundup(2 * 8 - 1, 256)
-    cu = torch.arange(0, 8 * (B + 1), 8, dtype=torch.int32, device=dev)
     x, y = t(256, 64), t(512, 64)         # xsim: 256 x 512 rows of dimension 64
     calls = {
         "sb_encoder_forward": lambda: lib.sb_encoder_forward(
@@ -63,8 +64,8 @@ def test_too_small_workspace_is_rejected(engines, cuda_device):
             decoder._handle, t(R, dtype=torch.int64), t(R, max_len, dtype=torch.int32), 0, n, beam, max_len, t(R, 16),
             t(R, 16, dtype=torch.int32), t(R), None, None, w, 1, stream),
         "sb_speech_encoder_forward": lambda: lib.sb_speech_encoder_forward(
-            speech._handle, t(B, 2 * 8, 80), 2 * 8, cu.data_ptr(), lens, B, t(rows, D, dtype=torch.bfloat16), rows,
-            t(B, D), None, w, 1, stream),
+            speech._handle, t(B, 2 * 8, 80), 2 * 8, lens, B, t(rows, D, dtype=torch.bfloat16), rows, t(B, D), None, w, 1,
+            stream),
         "sb_xsim_knn": lambda: lib.sb_xsim_knn(
             x, y, 256, 512, 64, 4, t(256, 4, dtype=torch.float64), t(256, 4, dtype=torch.int32), w, 1, stream),
         "sb_xsim_knn_bidir": lambda: lib.sb_xsim_knn_bidir(
@@ -129,49 +130,77 @@ def laser2(native_lib, cuda_device):
                                              num_layers=cfg.num_layers, bidirectional=cfg.bidirectional), sd, cuda_device)
 
 
-@pytest.mark.parametrize("engine", ["text_encoder", "laser2"])
+@pytest.mark.parametrize("engine", ["text_encoder", "laser2", "speech"])
 def test_a_burst_that_laps_the_staging_ring(engines, laser2, cuda_device, engine):
-    """17 forwards, more than twice the ring's 8 slots, enqueued on one stream behind a sleeping kernel with no host
-    synchronise, so the host laps the ring while the first forwards still wait: every output is bitwise that of the same
-    batch run on its own.  One out-of-range id in a middle forward makes check_inputs raise once; that check clears it."""
+    """17 forwards, more than twice the ring's 8 slots, enqueued on one stream behind a sleeping kernel.  An event recorded
+    right after the sleep is still pending once the first 8 are enqueued, so none of them synchronised with the stream.
+    The ninth reuses the first one's slot, so it must wait until that forward's copy has run: the host laps the ring only
+    as fast as the stream frees its slots.  Every output is bitwise that of the same batch run on its own.  For the token
+    engines, one out-of-range id in a middle forward makes check_inputs raise once; that check clears it.  The speech
+    batches are ragged but each has one utterance of the longest length, so the relative-position table is built once,
+    during the warm-up."""
     from sonar_b200 import PaddingMask, SequenceBatch
 
-    burst, max_batch, S = 17, 48, 40
+    burst, slots, max_batch, S = 17, 8, 48, 40
     dev = cuda_device
-    if engine == "text_encoder":
-        model = engines[0]
-
-        def run(ids, lens):
-            return model(SequenceBatch(ids, PaddingMask(torch.tensor(lens), S, lens))).sentence_embeddings
-    else:
-        model = laser2
-
-        def run(ids, lens):
-            return model(ids, torch.tensor(lens))
-
     g = torch.Generator().manual_seed(17)
+    if engine == "speech":
+        model = engines[2]
+
+        def make(lens):
+            return torch.randn((len(lens), 2 * S, 80), generator=g)
+
+        def run(fb, lens):
+            frames = [2 * n for n in lens]
+            return model(SequenceBatch(fb, PaddingMask(torch.tensor(frames), 2 * S, frames))).sentence_embeddings
+    else:
+        def make(lens):
+            ids = torch.ones((len(lens), S), dtype=torch.int64)  # pad_idx 1
+            for i, n in enumerate(lens):
+                ids[i, :n] = torch.randint(4, VOCAB, (n,), generator=g)
+            return ids
+
+        if engine == "text_encoder":
+            model = engines[0]
+
+            def run(ids, lens):
+                return model(SequenceBatch(ids, PaddingMask(torch.tensor(lens), S, lens))).sentence_embeddings
+        else:
+            model = laser2
+
+            def run(ids, lens):
+                return model(ids, torch.tensor(lens))
+
     batches = []
     for _ in range(burst):
         lens = torch.randint(1, S + 1, (int(torch.randint(1, max_batch + 1, (1,), generator=g)),), generator=g).tolist()
-        ids = torch.ones((len(lens), S), dtype=torch.int64)  # pad_idx 1
-        for i, n in enumerate(lens):
-            ids[i, :n] = torch.randint(4, VOCAB, (n,), generator=g)
-        batches.append((ids.to(dev), lens))  # on the device already: the wrappers make no blocking copy
+        if engine == "speech":
+            lens[int(torch.randint(0, len(lens), (1,), generator=g))] = S
+        batches.append((make(lens).to(dev), lens))  # on the device already: the wrappers make no blocking copy
     assert len({tuple(lens) for _, lens in batches}) == burst
-    batches[burst // 2][0][0, 0] = VOCAB
+    if engine != "speech":
+        batches[burst // 2][0][0, 0] = VOCAB
 
-    run(torch.full((max_batch, S), 5, dtype=torch.int64, device=dev), [S] * max_batch)  # grows the workspace once
+    run(make([S] * max_batch).to(dev), [S] * max_batch)  # grows the workspace once
     torch.cuda.synchronize(dev)
-    model.check_inputs()
-    torch.cuda._sleep(50_000_000)  # tens of milliseconds: the stream is busy while the host enqueues the burst
-    outs = [run(ids, lens) for ids, lens in batches]
-    torch.cuda.synchronize(dev)
-    with pytest.raises(ValueError, match="vocab"):
+    if engine != "speech":
         model.check_inputs()
-    model.check_inputs()
-    for i, (ids, lens) in enumerate(batches):
-        alone = run(ids, lens)
+    stream = torch.cuda.current_stream(dev)
+    torch.cuda._sleep(50_000_000)  # tens of milliseconds: the stream is busy while the host enqueues the burst
+    slept = torch.cuda.Event()
+    slept.record(stream)
+    outs = [run(x, lens) for x, lens in batches[:slots]]
+    assert not slept.query(), f"{engine}: a forward of the burst waited for the stream"
+    outs += [run(x, lens) for x, lens in batches[slots:]]
+    torch.cuda.synchronize(dev)
+    if engine != "speech":
+        with pytest.raises(ValueError, match="vocab"):
+            model.check_inputs()
+        model.check_inputs()
+    for i, (x, lens) in enumerate(batches):
+        alone = run(x, lens)
         torch.cuda.synchronize(dev)
         assert torch.equal(outs[i], alone), f"{engine}: forward {i} of the burst"
-    with pytest.raises(ValueError, match="vocab"):  # set again by the out-of-range batch on its own
-        model.check_inputs()
+    if engine != "speech":
+        with pytest.raises(ValueError, match="vocab"):  # set again by the out-of-range batch on its own
+            model.check_inputs()
